@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — POA windows/s (BASELINE.json metric) on B200, one process per GPU.
+"""bench.py — POA windows/s (BASELINE.md metric) on H100, one process per GPU.
 
-  python bench.py [--config 2|3|4|5] [--gpus N] [--steps K] [--warmup W]   our arm (sm_100a kernels via the C ABI)
+  python bench.py [--config 2|3|4|5] [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   our arm (sm_90a kernels via the C ABI)
   python bench.py --impl reference [--config ...] ...                      the reference's own CPU path (oracle/_ref)
   torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N             one rank per GPU
 
-Workloads (BASELINE.json `configs`; the default is config 2, the one the metric is quoted on at one GPU):
+Workloads (BASELINE.md; the default is config 2, the one the metric is quoted on at one GPU):
   2  synthetic 10k windows per GPU, w=500, 32 layers, 12 % ONT-like error, 3/-5/-4, full matrix   (weak scaling)
   3  synthetic 100k windows IN TOTAL, same shape, racon -b (banded), one stream cut into contiguous cost-balanced
      ranges, one per rank (SURVEY.md §8e)                                                          (strong scaling)
@@ -74,22 +74,11 @@ def measured_hbm_peak():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(cfg_id):
-    """Per-launch DRAM bytes of the POA kernel from the committed ncu --set full capture of this config, if any."""
-    path = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        with open(path) as f:
-            t = json.load(f)
-        return t.get("config%d" % cfg_id, t if cfg_id == 2 else None)
-    except Exception:
-        return None
+        return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -175,7 +164,7 @@ def config_key(cfg, args, banded=None):
     that the driver compares like with like; what THIS run did beyond that (window counts, batch objects, host binding,
     checksums ...) goes into the line's `run` object."""
     return {"workload": cfg["workload"], "baseline_config": args.config,
-            "l2": "GPU arm: a step's inputs (hundreds of MB) + DP scratch (tens of GB) exceed the 126 MB L2, no explicit flush; "
+            "l2": "GPU arm: a step's inputs (hundreds of MB) + DP scratch (tens of GB) exceed the 50 MB L2, no explicit flush; "
                   "reference arm: host cores, bounded sample of the same windows"}
 
 
@@ -372,6 +361,8 @@ def main():
     ap.add_argument("--internal-by-reference", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--e2e-batches", type=int, default=2,
                     help="batch objects the end-to-end arm cycles through (racon's -c/--cudapoa-batches)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy, for comparing two builds")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -497,6 +488,12 @@ def main():
     clocks = sampler.stop() if rank == 0 else None
     total_ms = ev0.elapsed_time(ev1)
     gpu_launches = batch.info()["launches"] + batch2.info()["launches"] - launches0
+    if args.dump_outputs:
+        last_batch = batch2 if args.steps % 2 == 0 and args.steps > 0 else batch   # the object of the last timed step
+        last_batch.download()
+        last_batch.sync()
+        dump_outputs(os.path.join(args.dump_outputs, "rank%d" % rank) if distributed else args.dump_outputs,
+                     *last_batch.fetch_all(stride))
     batch2.close()
     forced = None
     if banded:
@@ -636,7 +633,6 @@ def main():
         value = n_total / (ms_per_step * 1e-3)
         kern_avg_ms = sum(kern_ms) / len(kern_ms)
         achieved = alg_bytes / (kern_avg_ms * 1e-3) / 1e9
-        traffic = ncu_traffic(args.config)
         line = {
             "metric": cfg["metric"], "value": value, "unit": "windows/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": cfg["scaling"],
@@ -645,7 +641,7 @@ def main():
             "run": dict({"windows_rank0": n,
                             "window_len": wl, "banded": banded,
                             "parallelism": "windows sharded across %d GPU(s), no data-path collective" % world,
-                            "l2": "inputs (%.0f MB) + per-step DP scratch (>> 126 MB) exceed L2; no explicit flush"
+                            "l2": "inputs (%.0f MB) + per-step DP scratch (>> 50 MB) exceed L2; no explicit flush"
                                   % (io["h2d_bytes"] / 1e6),
                             "steps_overlap": "timed steps alternate between two resident batch objects on two streams; "
                                              "roofline.kernel_ms is an isolated launch",
@@ -665,8 +661,7 @@ def main():
             "gpu_launches": int(gpu_launches),
             "clocks": clocks,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": (traffic or {}).get("dram_bytes_per_launch"),
-                         "traffic_source": (traffic or {}).get("source"),
+                         "frac": achieved / peak,
                          "kernel": "rp_poa_kernel", "kernel_ms": kern_avg_ms,
                          "achieved_overlapped": alg_bytes / (ms_per_step * 1e-3) / 1e9 * (n / max(1, n_total / world)),
                          "algorithmic_bytes_per_launch": alg_bytes,
@@ -707,6 +702,26 @@ def main():
         else:
             store.wait(["bench_baselines_done"], datetime.timedelta(minutes=20))
         dist.destroy_process_group()
+
+
+def dump_outputs(path, out, lens, pol, st, limit_bytes=64 << 20):
+    """The results a caller of the timed path receives for its windows (consensus, polished flag, per-window status), as
+    float32 .npy files: consensus.npy holds the consensus bases (ASCII codes) of the windows in window_index.npy back to
+    back, consensus_length.npy their lengths.  When the consensus of every window would exceed limit_bytes, the windows
+    are a fixed seeded sample (the same one for the same workload)."""
+    import numpy as np
+    n = len(lens)
+    idx = np.arange(n)
+    per_window = 4 * (lens.astype(np.int64) + 4)
+    if per_window.sum() > limit_bytes:
+        order = np.random.default_rng(20240601).permutation(n)
+        idx = np.sort(order[:int(np.searchsorted(np.cumsum(per_window[order]), limit_bytes, side="right"))])
+    os.makedirs(path, exist_ok=True)
+    cons = [out[i, :lens[i]] for i in idx]
+    arrays = {"window_index": idx, "consensus_length": lens[idx], "polished": pol[idx], "status": st[idx],
+              "consensus": np.concatenate(cons) if cons else np.zeros(0)}
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), np.asarray(a, dtype=np.float32))
 
 
 def run_group(cmd, timeout, **kw):

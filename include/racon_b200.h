@@ -1,5 +1,5 @@
 /*
- * racon_b200.h — C ABI of the B200-native POA consensus / pre-alignment hot path.
+ * racon_b200.h — C ABI of the CUDA-native (sm_90a) POA consensus / pre-alignment hot path.
  *
  * Drop-in boundary for racon's GPU batch objects (SURVEY.md §8b).  Every entry point names the
  * reference interface it replaces; INTEGRATION.md shows the shim a racon maintainer adds in

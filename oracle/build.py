@@ -25,7 +25,7 @@ def build_ref():
 
 
 def build_ref_cudapoa():
-    """The reference's own GPU path (GenomeWorks cudapoa) compiled unmodified for sm_100 — timing baseline only."""
+    """The reference's own GPU path (GenomeWorks cudapoa) compiled unmodified for sm_90 — timing baseline only."""
     out = os.path.join(HERE, "_ref", "libref_cudapoa.so")
     if os.path.isdir("/root/reference/vendor/GenomeWorks/cudapoa/src"):
         try:
@@ -33,6 +33,13 @@ def build_ref_cudapoa():
         except RuntimeError as e:  # a baseline, not a checker: its absence is reported by bench.py, not fatal
             print("[oracle] reference cudapoa not built: %s" % str(e)[:500])
     return out if os.path.exists(out) else None
+
+
+def build_integration():
+    """The unmodified reference host linked against the product library (oracle/_ref/integration/racon, racon_goldens)."""
+    out = os.path.join(HERE, "_ref", "integration")
+    _make("integration")   # keeps what is there when the reference sources are absent
+    return out if os.path.isdir(out) else None
 
 
 def build_refpol():

@@ -31,7 +31,7 @@ def main():
         warm = ws.subset(range(min(400, a.windows)))
         ob.ref_cudapoa_multi(warm, banded=a.banded, n_devices=a.devices, batches_per_device=a.batches)
         ok, wall = ob.ref_cudapoa_multi(ws, banded=a.banded, n_devices=a.devices, batches_per_device=a.batches)
-        print(json.dumps({"kind": "reference GPU path: GenomeWorks cudapoa (unmodified, sm_100, %s), %d batch objects on "
+        print(json.dumps({"kind": "reference GPU path: GenomeWorks cudapoa (unmodified, sm_90, %s), %d batch objects on "
                                   "each of %d GPU(s), one host thread per batch object, as CUDAPolisher::polish"
                                   % (band, a.batches, a.devices),
                           "n_gpus": a.devices, "batches_per_gpu": a.batches, "windows": a.windows, "windows_ok": ok,
@@ -39,7 +39,7 @@ def main():
         return
     ob.ref_cudapoa_consensus(ws.subset(range(min(200, a.windows))), banded=a.banded, device=a.device)   # warm-up
     cons, ok, wall, gpu = ob.ref_cudapoa_consensus(ws, banded=a.banded, device=a.device)
-    print(json.dumps({"kind": "reference GPU path: GenomeWorks cudapoa (unmodified, sm_100, %s), driven as "
+    print(json.dumps({"kind": "reference GPU path: GenomeWorks cudapoa (unmodified, sm_90, %s), driven as "
                               "CUDABatchProcessor does" % band,
                       "windows": a.windows, "windows_ok": ok, "value": a.windows / wall, "unit": "windows/s",
                       "wall_s": wall, "gpu_call_s": gpu, "value_gpu_calls_only": a.windows / gpu if gpu else None,

@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI (include/racon_b200.h) — used by tests/, bench.py and __graft_entry__.py.
 
-The product is libracon_b200.so (C ABI + sm_100a kernels + C++ host mirror); this module only calls it.
+The product is libracon_b200.so (C ABI + sm_90a kernels + C++ host mirror); this module only calls it.
 Loading fails loudly when the library is missing; creating a batch fails loudly without a CUDA device.
 """
 import ctypes as C

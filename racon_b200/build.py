@@ -1,6 +1,6 @@
-"""Build helpers: every native artefact is built IN-TREE so it travels to the GPU box.
+"""Build helpers: every native artefact is built IN-TREE (racon_b200/lib/), next to the sources that load it.
 
-  libracon_b200.so       — the product: C-ABI (include/racon_b200.h) + sm_100a CUDA kernels, nothing else
+  libracon_b200.so       — the product: C-ABI (include/racon_b200.h) + sm_90a CUDA kernels, nothing else
   libracon_b200_host.so  — C++ host layer above the C ABI (racon_b200::Window / BatchProcessor / BatchAligner / Polisher,
                            the reference interface restated; reads_io: FASTA/FASTQ/PAF/MHAP/SAM input) + the rp_mirror_* hooks tests/ and
                            bench.py drive it with;
@@ -19,7 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "racon_b200", "csrc")
 LIBDIR = os.path.join(ROOT, "racon_b200", "lib")
 
-NVCC_ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _newer(target, sources):
@@ -65,7 +65,7 @@ def nvcc_path():
 
 
 def build_cuda(force=False, verbose=False):
-    """Compile the product library for sm_100a (cross-compiles without a GPU)."""
+    """Compile the product library for sm_90a (cross-compiles without a GPU)."""
     os.makedirs(LIBDIR, exist_ok=True)
     out = os.path.join(LIBDIR, "libracon_b200.so")
     cu = [os.path.join(CSRC, "rp_api.cu")]

@@ -44,7 +44,7 @@ inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
     std::strcpy(p->name, "host simulation");
     const char* e = std::getenv("RP_SIM_SMS");
     p->multiProcessorCount = e ? std::atoi(e) : 2;        // a small "GPU": a handful of workers, several waves per batch
-    p->sharedMemPerMultiprocessor = 233472;                // sm_100: 228 KB
+    p->sharedMemPerMultiprocessor = 233472;                // sm_90: 228 KB
     p->sharedMemPerBlockOptin = 232448;                    // 227 KB
     p->totalGlobalMem = size_t(8) << 30;
     return cudaSuccess;

@@ -1,5 +1,5 @@
 /*
- * poa_core.cuh — B200-native per-window partial-order-alignment consensus (device code).
+ * poa_core.cuh — CUDA-native (sm_90a) per-window partial-order-alignment consensus (device code).
  *
  * What the reference does per window (Window::generate_consensus, /root/reference/src/window.cpp:65-149,
  * driving spoa: vendor/spoa/src/graph.cpp and sisd/simd alignment engines) is done here by ONE WARP per

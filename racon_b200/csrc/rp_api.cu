@@ -1,5 +1,5 @@
 /*
- * rp_api.cu — the C ABI (include/racon_b200.h) over the sm_100a kernels.  Product library
+ * rp_api.cu — the C ABI (include/racon_b200.h) over the sm_90a kernels.  Product library
  * libracon_b200.so = this file alone (the C++ host layer above it, host_mirror.cpp, is a library of its own).
  * There is no CPU implementation behind these calls.
  *
@@ -172,9 +172,9 @@ template <int G, int KB>
 PoaKernel pick_kernel_g(int blocks_per_sm) {
     switch (blocks_per_sm) {
         case 2: return rp_poa_kernel<G, KB, 2>;
-        case 3: return rp_poa_kernel<G, KB, 3>;
+        case 4: return rp_poa_kernel<G, KB, 4>;
         case 6: return rp_poa_kernel<G, KB, 6>;
-        default: return rp_poa_kernel<G, KB, 4>;
+        default: return rp_poa_kernel<G, KB, 3>;
     }
 }
 template <int KB>
@@ -190,7 +190,7 @@ PoaKernel pick_kernel(int group, int band_k, int blocks_per_sm) {
 #if defined(RP_ONLY_DEFAULT_KERNEL)
     /* development builds for SASS inspection (tools/sass_by_line.py --quick): one instantiation, seconds to compile */
     (void)group; (void)band_k; (void)blocks_per_sm;
-    return rp_poa_kernel<32, 16, 4>;
+    return rp_poa_kernel<32, 16, 3>;
 #else
     if (group == 32 && band_k == 4) return pick_kernel_narrow<4>(blocks_per_sm);
     if (group == 32 && band_k == 8) return pick_kernel_narrow<8>(blocks_per_sm);
@@ -208,6 +208,12 @@ __global__ void __launch_bounds__(256) rp_gather_kernel(rp::GatherParams P) {
     const uint32_t warps = gridDim.x * (blockDim.x >> 5);
     for (uint32_t s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); s < P.n_seqs; s += warps)
         rp::gather_sequence(P, s);
+}
+/* its grid: one warp per sequence, at most 8 blocks per SM of the device */
+uint32_t gather_blocks(int device, uint32_t n_seqs) {
+    int sms = 0;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms < 1) sms = 1;
+    return std::max<uint32_t>(1, std::min<uint32_t>(static_cast<uint32_t>(sms) * 8, (n_seqs + 7) / 8));
 }
 
 template <int kBlocksPerSm>
@@ -346,7 +352,7 @@ const char* rp_strerror(rp_status s) {
 
 const char* rp_last_error(void) { return g_last_error.c_str(); }
 
-const char* rp_version(void) { return "racon_b200 0.1 (sm_100a)"; }
+const char* rp_version(void) { return "racon_b200 0.1 (sm_90a)"; }
 
 int rp_device_count(void) {
     int n = 0;
@@ -428,9 +434,11 @@ static rp_status configure(rp_poa* p, uint32_t wl) {
     if (const char* e_a = getenv("RP_BAND_AUDIT")) p->P.debug_flags = atoi(e_a) ? 2u : 0u;
 
     /* launch shape: persistent blocks of 4 warps = 128/G lane groups, kBlocksPerSm blocks per SM.  Defaults measured on
-     * B200 (profiles/README.md, round 2): full matrix: 32 lanes per window, 16 columns per lane, 4 blocks/SM; banded
-     * (-b): 32 lanes x 8 columns = a 256-column band (the width of cudapoa's static band) — four packed registers per
-     * row instead of eight.  RP_POA_BAND_K=4 selects a 128-column band (faster on clean data, refuses more often). */
+     * the H100 (tools/tune_poa.py, 10 000 windows of bench config 2): full matrix: 32 lanes per window, 16 columns per
+     * lane, 3 blocks/SM — at 4 blocks/SM the 128-register cap makes ptxas spill on sm_90a and the kernel is ~3 % slower;
+     * banded (-b): 32 lanes x 8 columns = a 256-column band (the width of cudapoa's static band) — four packed registers
+     * per row instead of eight — at 5 blocks/SM.  RP_POA_BAND_K=4 selects a 128-column band (faster on clean data,
+     * refuses more often). */
     int group = 32;
     if (const char* e_g = getenv("RP_POA_GROUP")) group = atoi(e_g);
     if (group != 8 && group != 16 && group != 32) group = 32;
@@ -444,10 +452,10 @@ static rp_status configure(rp_poa* p, uint32_t wl) {
     const bool band_forced = getenv("RP_POA_BAND_K") != nullptr || getenv("RP_POA_GROUP") != nullptr;
     p->P.banded = (banded && (band_forced || wl >= kBandPaysFromWindowLength)) ? 1 : 0;
     if (!p->P.banded) band_k = 16;
-    int bps = band_k == 16 ? 4 : 5;
+    int bps = band_k == 16 ? 3 : 5;
     if (const char* e_bps = getenv("RP_BLOCKS_PER_SM")) bps = atoi(e_bps);
     if (band_k == 16) {
-        if (bps != 2 && bps != 3 && bps != 6) bps = 4;
+        if (bps != 2 && bps != 4 && bps != 6) bps = 3;
     } else if (bps != 4 && bps != 6 && bps != 8) {
         bps = 5;
     }
@@ -920,8 +928,7 @@ rp_status rp_poa_upload(rp_poa* p) {
 #if defined(RP_HOST_SIM)
         rp_gather_kernel(G, SimLaunch{1, 256});
 #else
-        const uint32_t blocks = std::max<uint32_t>(1, std::min<uint32_t>(148 * 8, (G.n_seqs + 7) / 8));
-        rp_gather_kernel<<<blocks, 256, 0, p->stream>>>(G);
+        rp_gather_kernel<<<gather_blocks(p->device, G.n_seqs), 256, 0, p->stream>>>(G);
         RP_CUDA(cudaGetLastError());
 #endif
         p->gather_launches += 1;
@@ -1380,8 +1387,7 @@ rp_status rp_aln_upload(rp_aln* a) {
 #if defined(RP_HOST_SIM)
             rp_gather_kernel(G, SimLaunch{1, 256});
 #else
-            const uint32_t blocks = std::max<uint32_t>(1, std::min<uint32_t>(148 * 8, (G.n_seqs + 7) / 8));
-            rp_gather_kernel<<<blocks, 256, 0, a->stream>>>(G);
+            rp_gather_kernel<<<gather_blocks(a->device, G.n_seqs), 256, 0, a->stream>>>(G);
             RP_CUDA(cudaGetLastError());
 #endif
         }

@@ -2,7 +2,7 @@
  * rp_warp.cuh — the warp-level vocabulary the POA/Myers device code is written in.
  *
  * Two builds of the SAME device code:
- *   nvcc (sm_100a)         : thin wrappers over __shfl_sync / __ballot_sync / DPX packed-int16 ops
+ *   nvcc (sm_90a)          : thin wrappers over __shfl_sync / __ballot_sync / DPX packed-int16 ops
  *                            (VIADDMNMX.S16x2 via __viaddmax_s16x2, PRMT via __byte_perm).
  *   g++ -DRP_HOST_SIM=1    : TEST-ONLY simulation — one simulated warp = 32 cooperative fibres
  *                            (ucontext) that meet at every collective.  It lets tests/ run the device
@@ -200,7 +200,7 @@ inline uint32_t byte_perm(uint32_t a, uint32_t b, uint32_t sel) {
 }
 
 #else
-/* ------------------------------------------------------------------ sm_100a */
+/* ------------------------------------------------------------------ sm_90a */
 RP_DEV int lane_id() { return static_cast<int>(threadIdx.x & 31); }
 RP_DEV void syncwarp() { __syncwarp(); }
 /* 16-byte asynchronous global -> shared copy (LDGSTS): the data goes from HBM / L2 into shared memory without passing

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _device_count():
@@ -27,7 +27,7 @@ def pytest_collection_modifyitems(config, items):
         return
     if _device_count() > 0:
         return
-    skip = pytest.mark.skip(reason="no CUDA device: GPU parity tests run on the B200 box (pytest -m gpu)")
+    skip = pytest.mark.skip(reason="no CUDA device: GPU parity tests run on an H100 (pytest -m gpu)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C ABI, against the oracle,
+"""GPU parity tests (run on an H100): the CUDA path, called through the C ABI, against the oracle,
 the committed golden fixtures and the reference's known-answer checksums.  Integer/byte work => bit-exact."""
 import json
 import os

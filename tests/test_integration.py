@@ -1,13 +1,13 @@
 """The UNMODIFIED reference host (src/main.cpp, src/polisher.cpp, src/cuda/cudapolisher.cpp, ... compiled where they lie
-by integration/Makefile with -DCUDA_ENABLED) linked against libracon_b200.so through integration/cudabatch.cpp and
-integration/cudaaligner.cpp, run on the reference's own sample files.
+by `make -C oracle integration` with -DCUDA_ENABLED) linked against libracon_b200.so through integration/cudabatch.cpp and
+integration/cudaaligner.cpp, run on the reference's own sample files (tests/golden/data).
 
   * `racon -c 1 [-b] [--cudaaligner-batches 1]` prints exactly what the reference's CPU build prints (md5 of stdout);
   * the reference's CUDA test cases (test/racon_test.cpp:297-507) reach the CPU goldens of test/racon_test.cpp:86-295 —
     the reference's own CUDA build does not (it carries separate goldens: 1385, 1607, 1541, 1661, 4168, 1361, 397185 ...).
 
-The binaries and the sample files are built/copied here (CPU container, where /root/reference exists) into
-integration/_build/, which travels to the GPU box with the repo snapshot."""
+The binaries are built with the other reference binaries into oracle/_ref/integration/, where the reference sources
+exist."""
 import hashlib
 import json
 import os
@@ -15,11 +15,13 @@ import subprocess
 
 import pytest
 
+from tests import util
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BUILD = os.path.join(ROOT, "integration", "_build")
+BUILD = os.path.join(ROOT, "oracle", "_ref", "integration")
 RACON = os.path.join(BUILD, "racon")
 GOLDENS = os.path.join(BUILD, "racon_goldens")
-DATA = os.path.join(BUILD, "data")
+DATA = util.sample_data_dir()
 
 # racon's stdout on the sample with default scores (SURVEY.md §8c: identical for 1/4/8 threads, SISD and AVX2 builds)
 MD5_DEFAULT = "b0e2a2788440a4982e544e2e9b3bf378"
@@ -41,8 +43,8 @@ CPU_GOLDENS = {
 
 
 def _need_build():
-    if not (os.path.exists(RACON) and os.path.exists(GOLDENS) and os.path.isdir(DATA)):
-        pytest.skip("integration/_build missing: run `make -C integration` where /root/reference exists")
+    if not (os.path.exists(RACON) and os.path.exists(GOLDENS)):
+        pytest.skip("oracle/_ref/integration missing: it is built where the reference sources exist")
 
 
 def test_integration_binaries_are_the_reference_host_linked_to_the_product_library():

@@ -302,7 +302,7 @@ def test_sim_narrow_band_refusal_and_other_scores():
 
 
 def test_sim_band_real_windows_whose_true_path_leaves_the_band():
-    """Two windows of the lambda -f run (unit scores) found on the B200 by tools/find_band_divergence.py: a layer's true
+    """Two windows of the lambda -f run (unit scores) found on the GPU by tools/find_band_divergence.py: a layer's true
     alignment runs 70-130 columns away from the band's centre line while an in-band path of almost the same score keeps
     every margin — the band result used to be accepted and the consensus differed from the reference's.  The acceptance
     check's alignment-quality rule (kBandJunkLimit) now refuses those band results; the on-device full-matrix redo makes the

@@ -13,8 +13,7 @@ from racon_b200 import api
 from tests import util
 from tests.test_reads_io import CASES, DATA, GOLD
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not os.path.isdir(DATA), reason="integration/_build/data missing")]
+pytestmark = pytest.mark.gpu
 
 
 def _records(path):

@@ -1,5 +1,9 @@
 """Shared test helpers: random window makers (numpy RNG; test-only) and checker access."""
+import atexit
+import os
+import shutil
 import struct
+import tempfile
 import zlib
 
 import numpy as np
@@ -7,6 +11,39 @@ import numpy as np
 from racon_b200 import windows
 
 BASES = b"ACGT"
+GOLDEN_DATA = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "data")
+_sample_dir = []
+
+
+def sample_data_dir():
+    """The reference's lambda-phage sample files (tests/golden/data) as a directory of whole files.  No stored file exceeds
+    1 MB, so the larger ones are kept as NAME.part0, NAME.part1 ...: they are joined here, into a temporary directory that
+    is removed when the process exits."""
+    if not _sample_dir:
+        d = tempfile.mkdtemp(prefix="racon_b200_samples_")
+        atexit.register(shutil.rmtree, d, True)
+        for f in sorted(os.listdir(GOLDEN_DATA)):
+            with open(os.path.join(GOLDEN_DATA, f), "rb") as src, open(os.path.join(d, f.rsplit(".part", 1)[0]), "ab") as dst:
+                dst.write(src.read())
+        _sample_dir.append(d)
+    return _sample_dir[0]
+
+
+def ref_answers():
+    """What the unmodified reference answered on the oracle tests' inputs (tests/golden/make_ref_answers.py)."""
+    import json
+    with open(os.path.join(os.path.dirname(GOLDEN_DATA), "ref_answers.json")) as f:
+        return json.load(f)
+
+
+def cigar_answer(res):
+    """(CIGAR, edit distance) as stored: [CRC-32 of the CIGAR, edit distance]."""
+    return [zlib.crc32(res[0].encode()), int(res[1])]
+
+
+def consensus_answer(cons, polished):
+    """Per window, as stored: [CRC-32 of the consensus, polished flag]."""
+    return [[zlib.crc32(c), int(p)] for c, p in zip(cons, polished)]
 
 
 def mutate(rng, t, err, alphabet=BASES):

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Static instruction counts of one kernel by source line / function, from the SASS (no GPU needed).
 
-  python tools/sass_by_line.py [--kernel 'rp_poa_kernelILi32ELi16ELi4E'] [--lines poa_core.cuh:1300-1520] [--top 40]
+  python tools/sass_by_line.py [--kernel 'rp_poa_kernelILi32ELi16ELi3E'] [--lines poa_core.cuh:1300-1520] [--top 40]
 
-cuobjdump extracts the sm_100a cubin of racon_b200/lib/libracon_b200.so, `nvdisasm -g` annotates every instruction with
+cuobjdump extracts the sm_90a cubin of racon_b200/lib/libracon_b200.so, `nvdisasm -g` annotates every instruction with
 the source line it was generated for (the library is built with -lineinfo).  The counts are STATIC (instructions in the
 binary, not executed ones): they are what a change of the source can be checked against before any GPU time is spent —
 together with `ncu_by_line.py`'s dynamic counts from a capture.  --lines prints the listing of a source range."""
@@ -18,10 +18,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def disassemble(lib, kernel):
-    tmp = tempfile.mkdtemp(prefix="sass_")
-    subprocess.run(["cuobjdump", "-xelf", "all", lib], cwd=tmp, check=True, stdout=subprocess.DEVNULL)
-    cubin = [os.path.join(tmp, f) for f in os.listdir(tmp) if f.endswith(".cubin")][0]
-    out = subprocess.run(["nvdisasm", "-g", cubin], stdout=subprocess.PIPE, text=True, check=True).stdout
+    with tempfile.TemporaryDirectory(prefix="sass_") as tmp:
+        subprocess.run(["cuobjdump", "-xelf", "all", lib], cwd=tmp, check=True, stdout=subprocess.DEVNULL)
+        cubin = [os.path.join(tmp, f) for f in os.listdir(tmp) if f.endswith(".cubin")][0]
+        out = subprocess.run(["nvdisasm", "-g", cubin], stdout=subprocess.PIPE, text=True, check=True).stdout
     sect, keep = None, []
     for line in out.splitlines():
         m = re.match(r"\s*\.section\s+\.text\.(\S+?),", line)
@@ -38,7 +38,7 @@ def disassemble(lib, kernel):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", default=os.path.join(ROOT, "racon_b200", "lib", "libracon_b200.so"))
-    ap.add_argument("--kernel", default="rp_poa_kernelILi32ELi16ELi4E")
+    ap.add_argument("--kernel", default="rp_poa_kernelILi32ELi16ELi3E")
     ap.add_argument("--lines", help="file.cuh:first-last : print the SASS generated for that source range")
     ap.add_argument("--top", type=int, default=40)
     ap.add_argument("--range", help="lo-hi (hex addresses): plain listing of that address range, source lines beside it")

@@ -34,7 +34,7 @@ def main():
         os.environ["RP_BLOCKS_PER_SM"] = str(bps)
         os.environ["RP_POA_BAND_K"] = str(k)
         try:
-            b = api.PoaBatch(device=0, window_length=args.wlen, banded=bool(banded), mem_bytes=int(60e9))
+            b = api.PoaBatch(device=0, window_length=args.wlen, banded=bool(banded), mem_bytes=int(30e9))
             st = torch.cuda.current_stream()
             b.set_stream(st.cuda_stream)
             assert b.add_window_set(ws) == ws.n_windows
@@ -63,7 +63,7 @@ def main():
                    "bad_status": int((status != 0).sum()), "fnv200": ck, "same_as_first": full == ref,
                    "band": bi}
             if args.two_streams:
-                b2 = api.PoaBatch(device=0, window_length=args.wlen, banded=bool(banded), mem_bytes=int(60e9))
+                b2 = api.PoaBatch(device=0, window_length=args.wlen, banded=bool(banded), mem_bytes=int(30e9))
                 s2 = torch.cuda.Stream()
                 b2.set_stream(s2.cuda_stream)
                 assert b2.add_window_set(ws) == ws.n_windows

@@ -1,4 +1,4 @@
-// Microbenchmark: issue rate of the integer ops the POA DP inner loop could be built from (sm_100a).
+// Microbenchmark: issue rate of the integer ops the POA DP inner loop could be built from (sm_90a).
 // Prints warp-instructions per clock per SM for each op at 4, 8, 16 warps per SM.
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -35,21 +35,22 @@ __global__ void k(unsigned* out, int iters, unsigned seed) {
 
 template <int OP>
 void run(const char* name, int instr_per_op) {
-    unsigned* out;
-    cudaMalloc(&out, 148 * 1024 * 4);
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, 0);
+    const int sms = prop.multiProcessorCount;   // one block per SM
+    unsigned* out;
+    cudaMalloc(&out, sms * 1024 * 4);
     int clk_khz;
     cudaDeviceGetAttribute(&clk_khz, cudaDevAttrClockRate, 0);
     for (int warps = 4; warps <= 32; warps *= 2) {
         int iters = 20000;
-        k<OP><<<148, warps * 32>>>(out, 100, 1);
+        k<OP><<<sms, warps * 32>>>(out, 100, 1);
         cudaDeviceSynchronize();
         cudaEvent_t e0, e1;
         cudaEventCreate(&e0);
         cudaEventCreate(&e1);
         cudaEventRecord(e0);
-        k<OP><<<148, warps * 32>>>(out, iters, 1);
+        k<OP><<<sms, warps * 32>>>(out, iters, 1);
         cudaEventRecord(e1);
         cudaEventSynchronize(e1);
         float ms;
