@@ -20,6 +20,84 @@ class RaconB200Error(RuntimeError):
     pass
 
 
+_vp, _u32, _u64, _int, _st = C.c_void_p, C.c_uint32, C.c_uint64, C.c_int, C.c_int32
+_i8, _str, _size = C.c_int8, C.c_char_p, C.c_size_t
+
+# name: (restype, argtypes) of every function of the C ABI (include/racon_b200.h)
+SIGNATURES = {
+    "rp_strerror": (_str, [_st]),
+    "rp_last_error": (_str, []),
+    "rp_device_count": (_int, []),
+    "rp_version": (_str, []),
+    "rp_poa_create": (_st, [C.POINTER(_vp), _int, _size, _i8, _i8, _i8, _int, _u32, _u32]),
+    "rp_poa_destroy": (None, [_vp]),
+    "rp_poa_add_window": (_st, [_vp, _u32, _vp, _vp, _vp, _vp, _vp, _int, _int]),
+    "rp_reads_create": (_st, [C.POINTER(_vp), _int, _u32, _vp, _vp, _vp]),
+    "rp_reads_destroy": (None, [_vp]),
+    "rp_reads_bytes": (_u64, [_vp]),
+    "rp_poa_add_window_refs": (_st, [_vp, _vp, _u32] + [_vp] * 6 + [_int, _int]),
+    "rp_poa_add_window_set_refs": (_st, [_vp, _vp, _u32, _u32] + [_vp] * 8 + [_int, _vp]),
+    "rp_poa_add_window_set": (_st, [_vp, _u32, _u32] + [_vp] * 8 + [_int, _vp]),
+    "rp_poa_size": (_u32, [_vp]),
+    "rp_poa_run": (_st, [_vp]),
+    "rp_poa_sync": (_st, [_vp]),
+    "rp_poa_upload": (_st, [_vp]),
+    "rp_poa_launch": (_st, [_vp]),
+    "rp_poa_download": (_st, [_vp]),
+    "rp_poa_fetch": (_st, [_vp, _u32, _vp, _vp, _vp, _vp]),
+    "rp_poa_window_status": (_st, [_vp, _u32, _vp]),
+    "rp_poa_fetch_all": (_st, [_vp, _vp, _u32, _vp, _vp, _vp]),
+    "rp_poa_reset": (_st, [_vp]),
+    "rp_poa_set_stream": (_st, [_vp, _vp]),
+    "rp_poa_info": (_st, [_vp, _vp]),
+    "rp_poa_enable_counters": (_st, [_vp, _int]),
+    "rp_poa_band_info": (_st, [_vp, _vp]),
+    "rp_aln_create": (_st, [C.POINTER(_vp), _int, _size, _u32]),
+    "rp_aln_destroy": (None, [_vp]),
+    "rp_aln_add": (_st, [_vp, _str, _u32, _str, _u32]),
+    "rp_aln_set_window_length": (_st, [_vp, _u32]),
+    "rp_aln_add_overlap": (_st, [_vp, _str, _u32, _str, _u32, _u32, _u32]),
+    "rp_aln_add_overlap_ref": (_st, [_vp, _vp, _u32, _u32, _u32, _int, _u32, _u32, _u32]),
+    "rp_aln_fetch_breaking_points": (_st, [_vp, _u32, _vp, _vp]),
+    "rp_aln_size": (_u32, [_vp]),
+    "rp_aln_run": (_st, [_vp]),
+    "rp_aln_sync": (_st, [_vp]),
+    "rp_aln_upload": (_st, [_vp]),
+    "rp_aln_launch": (_st, [_vp]),
+    "rp_aln_download": (_st, [_vp]),
+    "rp_aln_fetch_cigar": (_st, [_vp, _u32, _vp, _vp, _vp, _vp]),
+    "rp_aln_reset": (_st, [_vp]),
+    "rp_aln_set_stream": (_st, [_vp, _vp]),
+    "rp_aln_info": (_st, [_vp, _vp]),
+}
+
+# the test hooks of the C++ host layer (libracon_b200_host.so, host_mirror.cpp / reads_io.cpp), bound when present
+HOST_SIGNATURES = {
+    "rp_mirror_align": (_int, [_u32, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _u32]),
+    "rp_mirror_consensus": (C.c_double, [_u32] + [_vp] * 8 + [_i8, _i8, _i8, _u32, _int, _u32, _vp, _u32, _vp, _vp]),
+    "rp_mirror_polisher_open": (_vp, [_u32, _vp, _vp, _vp, _vp, _u32, _int, _int, _u32, _vp, _u32, C.c_double, _int,
+                                      _i8, _i8, _i8, _u32]),
+    "rp_mirror_polisher_open_with_bp": (_vp, [_u32, _vp, _vp, _vp, _vp, _u32, _int, _int, _u32, _vp, _vp, _vp, _u32,
+                                              C.c_double]),
+    "rp_mirror_polisher_open_files": (_vp, [_str, _str, _str, _int, _u32, C.c_double, C.c_double, _int, _i8, _i8, _i8,
+                                            _u32, _int, _vp, _u32]),
+    "rp_mirror_polisher_counts": (None, [_vp, _vp]),
+    "rp_mirror_polisher_export": (None, [_vp] * 11),
+    "rp_mirror_polisher_polish": (_u32, [_vp, _int]),
+    "rp_mirror_polisher_window_consensus": (_u32, [_vp, _u32, _vp, _u32]),
+    "rp_mirror_polisher_polished": (_u64, [_vp, _u32, _vp, _vp, _u32, _vp, _u64]),
+    "rp_mirror_polisher_close": (None, [_vp]),
+    "rp_mirror_polisher_failed": (None, [_vp, _vp]),
+    "rp_mirror_polisher_stream_fasta": (_u32, [_vp, _int, _str, _str, _u64, _int, _int]),
+    "rp_mirror_format_fasta": (_u64, [_str, _str, _str, _u64, _str, _u64]),
+    "rp_mirror_input_open": (_vp, [_str, _str, _str, _int, C.c_double, _vp, _u32]),
+    "rp_mirror_input_counts": (None, [_vp, _vp]),
+    "rp_mirror_input_export": (None, [_vp] * 8),
+    "rp_mirror_input_cigar_breaking_points": (_u32, [_vp, _u32, _u32, _vp, _u32]),
+    "rp_mirror_input_close": (None, [_vp]),
+}
+
+
 def lib_path():
     return os.environ.get("RACON_B200_LIB") or os.path.join(build.LIBDIR, "libracon_b200.so")
 
@@ -39,87 +117,20 @@ def load(build_if_missing=True):
     if not os.path.exists(path):
         raise RaconB200Error("libracon_b200.so is missing: run __graft_entry__.build() (no CPU fallback exists)")
     lib = C.CDLL(path)
-    vp, u32, u64 = C.c_void_p, C.c_uint32, C.c_uint64
-    lib.rp_strerror.restype = C.c_char_p
-    lib.rp_strerror.argtypes = [C.c_int32]
-    lib.rp_last_error.restype = C.c_char_p
-    lib.rp_version.restype = C.c_char_p
-    lib.rp_device_count.restype = C.c_int
-    lib.rp_poa_create.restype = C.c_int32
-    lib.rp_poa_create.argtypes = [C.POINTER(vp), C.c_int, C.c_size_t, C.c_int8, C.c_int8, C.c_int8, C.c_int, u32, u32]
-    lib.rp_poa_destroy.restype = None
-    lib.rp_poa_destroy.argtypes = [vp]
-    lib.rp_poa_add_window.restype = C.c_int32
-    lib.rp_poa_add_window.argtypes = [vp, u32, vp, vp, vp, vp, vp, C.c_int, C.c_int]
-    lib.rp_poa_add_window_set.restype = C.c_int32
-    lib.rp_poa_add_window_set.argtypes = [vp, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp]
-    lib.rp_poa_size.restype = u32
-    lib.rp_poa_size.argtypes = [vp]
-    for name in ("rp_poa_run", "rp_poa_sync", "rp_poa_upload", "rp_poa_launch", "rp_poa_download", "rp_poa_reset"):
-        getattr(lib, name).restype = C.c_int32
-        getattr(lib, name).argtypes = [vp]
-    lib.rp_poa_fetch.restype = C.c_int32
-    lib.rp_poa_fetch.argtypes = [vp, u32, vp, vp, vp, vp]
-    lib.rp_poa_window_status.restype = C.c_int32
-    lib.rp_poa_window_status.argtypes = [vp, u32, vp]
-    lib.rp_poa_fetch_all.restype = C.c_int32
-    lib.rp_poa_fetch_all.argtypes = [vp, vp, u32, vp, vp, vp]
-    lib.rp_poa_set_stream.restype = C.c_int32
-    lib.rp_poa_set_stream.argtypes = [vp, vp]
-    lib.rp_poa_info.restype = C.c_int32
-    lib.rp_poa_info.argtypes = [vp, vp]
-    lib.rp_poa_enable_counters.restype = C.c_int32
-    lib.rp_poa_enable_counters.argtypes = [vp, C.c_int]
-    lib.rp_poa_band_info.restype = C.c_int32
-    lib.rp_poa_band_info.argtypes = [vp, vp]
-    _bind_aln(lib, C, vp, u32)
+    for name, (restype, argtypes) in SIGNATURES.items():
+        f = getattr(lib, name)
+        f.restype, f.argtypes = restype, argtypes
     # the C++ host layer and its hooks live in a library of their own (it links against the product, not vice versa)
     host_path = os.path.join(os.path.dirname(path), "libracon_b200_host.so")
     if os.path.exists(host_path):
         host = C.CDLL(host_path)
-        for name in ("rp_mirror_align", "rp_mirror_consensus", "rp_mirror_polisher_open", "rp_mirror_polisher_open_with_bp",
-                     "rp_mirror_polisher_counts", "rp_mirror_polisher_export", "rp_mirror_polisher_polish",
-                     "rp_mirror_polisher_window_consensus", "rp_mirror_polisher_polished", "rp_mirror_polisher_close",
-                     "rp_mirror_polisher_failed", "rp_mirror_format_fasta", "rp_mirror_polisher_stream_fasta",
-                     "rp_mirror_input_open", "rp_mirror_input_counts", "rp_mirror_input_export",
-                     "rp_mirror_input_cigar_breaking_points", "rp_mirror_input_close", "rp_mirror_polisher_open_files"):
+        for name, (restype, argtypes) in HOST_SIGNATURES.items():
             if hasattr(host, name):
-                setattr(lib, name, getattr(host, name))
-    if hasattr(lib, "rp_mirror_align"):
-        lib.rp_mirror_align.restype = C.c_int
-        lib.rp_mirror_align.argtypes = [u32, vp, vp, vp, vp, vp, u32, u32, vp, u32]
-    if hasattr(lib, "rp_mirror_consensus"):
-        lib.rp_mirror_consensus.restype = C.c_double
-        lib.rp_mirror_consensus.argtypes = [u32] + [vp] * 8 + [C.c_int8, C.c_int8, C.c_int8, u32, C.c_int, u32, vp,
-                                                               u32, vp, vp]
+                f = getattr(host, name)
+                f.restype, f.argtypes = restype, argtypes
+                setattr(lib, name, f)
     _lib = lib
     return lib
-
-
-def _bind_aln(lib, C, vp, u32):
-    lib.rp_aln_create.restype = C.c_int32
-    lib.rp_aln_create.argtypes = [C.POINTER(vp), C.c_int, C.c_size_t, u32]
-    lib.rp_aln_destroy.restype = None
-    lib.rp_aln_destroy.argtypes = [vp]
-    lib.rp_aln_add.restype = C.c_int32
-    lib.rp_aln_add.argtypes = [vp, C.c_char_p, u32, C.c_char_p, u32]
-    lib.rp_aln_set_window_length.restype = C.c_int32
-    lib.rp_aln_set_window_length.argtypes = [vp, u32]
-    lib.rp_aln_add_overlap.restype = C.c_int32
-    lib.rp_aln_add_overlap.argtypes = [vp, C.c_char_p, u32, C.c_char_p, u32, u32, u32]
-    lib.rp_aln_fetch_breaking_points.restype = C.c_int32
-    lib.rp_aln_fetch_breaking_points.argtypes = [vp, u32, vp, vp]
-    lib.rp_aln_size.restype = u32
-    lib.rp_aln_size.argtypes = [vp]
-    for name in ("rp_aln_run", "rp_aln_sync", "rp_aln_upload", "rp_aln_launch", "rp_aln_download", "rp_aln_reset"):
-        getattr(lib, name).restype = C.c_int32
-        getattr(lib, name).argtypes = [vp]
-    lib.rp_aln_fetch_cigar.restype = C.c_int32
-    lib.rp_aln_fetch_cigar.argtypes = [vp, u32, vp, vp, vp, vp]
-    lib.rp_aln_set_stream.restype = C.c_int32
-    lib.rp_aln_set_stream.argtypes = [vp, vp]
-    lib.rp_aln_info.restype = C.c_int32
-    lib.rp_aln_info.argtypes = [vp, vp]
 
 
 def _check(lib, st, what):
@@ -147,10 +158,7 @@ class ReadStore:
         ln = (C.c_uint32 * n)(*[len(x) for x in sequences])
         self._arrays = (sp, qp, ln)
         self.h = C.c_void_p()
-        f = self.lib.rp_reads_create
-        f.restype = C.c_int32
-        f.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
-        _check(self.lib, f(C.byref(self.h), device, n, sp, qp, ln), "rp_reads_create")
+        _check(self.lib, self.lib.rp_reads_create(C.byref(self.h), device, n, sp, qp, ln), "rp_reads_create")
 
     @classmethod
     def from_flat(cls, bases, seq_off, quals=None, seq_has_qual=None, device=0):
@@ -169,21 +177,15 @@ class ReadStore:
         self._keep = (bases, quals, ptrs, qptrs, ln)
         self._arrays = None
         self.h = C.c_void_p()
-        f = self.lib.rp_reads_create
-        f.restype = C.c_int32
-        f.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
-        _check(self.lib, f(C.byref(self.h), device, n, _ptr(ptrs), _ptr(qptrs), _ptr(ln)), "rp_reads_create")
+        _check(self.lib, self.lib.rp_reads_create(C.byref(self.h), device, n, _ptr(ptrs), _ptr(qptrs), _ptr(ln)),
+               "rp_reads_create")
         return self
 
     def device_bytes(self):
-        self.lib.rp_reads_bytes.restype = C.c_uint64
-        self.lib.rp_reads_bytes.argtypes = [C.c_void_p]
         return int(self.lib.rp_reads_bytes(self.h))
 
     def close(self):
         if self.h:
-            self.lib.rp_reads_destroy.restype = None
-            self.lib.rp_reads_destroy.argtypes = [C.c_void_p]
             self.lib.rp_reads_destroy(self.h)
             self.h = C.c_void_p()
 
@@ -252,11 +254,8 @@ class PoaBatch:
         cols = [np.ascontiguousarray(a[:, k].astype(np.uint32)) for k in (0, 1, 2)]
         rev = np.ascontiguousarray(a[:, 3].astype(np.uint8))
         bg, en = (np.ascontiguousarray(a[:, k].astype(np.uint32)) for k in (4, 5))
-        f = self.lib.rp_poa_add_window_refs
-        f.restype = C.c_int32
-        f.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32] + [C.c_void_p] * 6 + [C.c_int, C.c_int]
-        st = f(self.h, store.h, len(a), _ptr(cols[0]), _ptr(cols[1]), _ptr(cols[2]), _ptr(rev), _ptr(bg), _ptr(en),
-               window_type, 1 if trim else 0)
+        st = self.lib.rp_poa_add_window_refs(self.h, store.h, len(a), _ptr(cols[0]), _ptr(cols[1]), _ptr(cols[2]),
+                                             _ptr(rev), _ptr(bg), _ptr(en), window_type, 1 if trim else 0)
         return _check(self.lib, st, "rp_poa_add_window_refs")
 
     def add_window_set_refs(self, store, refs, first=0, count=None, trim=True):
@@ -264,13 +263,11 @@ class PoaBatch:
         per piece) + win_first (windows + 1) and optionally win_type.  Returns how many windows fit."""
         if count is None:
             count = len(refs["win_first"]) - 1 - first
-        f = self.lib.rp_poa_add_window_set_refs
-        f.restype = C.c_int32
-        f.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32] + [C.c_void_p] * 8 + [C.c_int, C.c_void_p]
         added = C.c_uint32(0)
-        st = f(self.h, store.h, first, count, _ptr(refs["seq_id"]), _ptr(refs["offset"]), _ptr(refs["length"]),
-               _ptr(refs.get("reverse")), _ptr(refs["begin"]), _ptr(refs["end"]), _ptr(refs["win_first"]),
-               _ptr(refs.get("win_type")), 1 if trim else 0, C.byref(added))
+        st = self.lib.rp_poa_add_window_set_refs(
+            self.h, store.h, first, count, _ptr(refs["seq_id"]), _ptr(refs["offset"]), _ptr(refs["length"]),
+            _ptr(refs.get("reverse")), _ptr(refs["begin"]), _ptr(refs["end"]), _ptr(refs["win_first"]),
+            _ptr(refs.get("win_type")), 1 if trim else 0, C.byref(added))
         _check(self.lib, st, "rp_poa_add_window_set_refs")
         return added.value
 
@@ -382,12 +379,9 @@ class AlnBatch:
         """The overlap named as slices of a device-resident ReadStore (rp_aln_add_overlap_ref): query = q_len bases of
         sequence q_id from q_start on (of its reverse complement when q_reverse), target = t_len bases of t_id from
         t_begin on.  False = batch full (like add)."""
-        f = self.lib.rp_aln_add_overlap_ref
-        f.restype = C.c_int32
-        f.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_uint32, C.c_uint32,
-                      C.c_uint32]
-        return _check(self.lib, f(self.h, store.h, q_id, q_start, q_len, 1 if q_reverse else 0, t_id, t_begin, t_len),
-                      "rp_aln_add_overlap_ref") == RP_OK
+        st = self.lib.rp_aln_add_overlap_ref(self.h, store.h, q_id, q_start, q_len, 1 if q_reverse else 0, t_id, t_begin,
+                                             t_len)
+        return _check(self.lib, st, "rp_aln_add_overlap_ref") == RP_OK
 
     def size(self):
         return self.lib.rp_aln_size(self.h)
@@ -490,22 +484,6 @@ class MirrorPolisher:
         (host logic only; no GPU needed, polish() is then not available)."""
         self.lib = load()
         L = self.lib
-        vp = C.c_void_p
-        L.rp_mirror_polisher_open.restype = vp
-        L.rp_mirror_polisher_open.argtypes = [C.c_uint32, vp, vp, vp, vp, C.c_uint32, C.c_int, C.c_int, C.c_uint32, vp,
-                                              C.c_uint32, C.c_double, C.c_int, C.c_int8, C.c_int8, C.c_int8, C.c_uint32]
-        L.rp_mirror_polisher_counts.restype = None
-        L.rp_mirror_polisher_counts.argtypes = [vp, vp]
-        L.rp_mirror_polisher_export.restype = None
-        L.rp_mirror_polisher_export.argtypes = [vp] * 11
-        L.rp_mirror_polisher_polish.restype = C.c_uint32
-        L.rp_mirror_polisher_polish.argtypes = [vp, C.c_int]
-        L.rp_mirror_polisher_window_consensus.restype = C.c_uint32
-        L.rp_mirror_polisher_window_consensus.argtypes = [vp, C.c_uint32, vp, C.c_uint32]
-        L.rp_mirror_polisher_polished.restype = C.c_uint64
-        L.rp_mirror_polisher_polished.argtypes = [vp, C.c_uint32, vp, vp, C.c_uint32, vp, C.c_uint64]
-        L.rp_mirror_polisher_close.restype = None
-        L.rp_mirror_polisher_close.argtypes = [vp]
         # keep the sequence bytes alive: the windows point into them
         self._bases = np.ascontiguousarray(np.frombuffer(bases, np.uint8))
         self._quals = np.ascontiguousarray(np.frombuffer(quals, np.uint8))
@@ -513,9 +491,6 @@ class MirrorPolisher:
         self._hq = np.ascontiguousarray(seq_has_qual, dtype=np.uint8)
         ov = np.ascontiguousarray(overlaps, dtype=np.uint32)
         if breaking_points is not None:
-            L.rp_mirror_polisher_open_with_bp.restype = vp
-            L.rp_mirror_polisher_open_with_bp.argtypes = [C.c_uint32, vp, vp, vp, vp, C.c_uint32, C.c_int, C.c_int,
-                                                          C.c_uint32, vp, vp, vp, C.c_uint32, C.c_double]
             bp_off = np.ascontiguousarray(breaking_points[0], dtype=np.uint64)
             bp = np.ascontiguousarray(breaking_points[1], dtype=np.uint32)
             self.h = L.rp_mirror_polisher_open_with_bp(len(self._off) - 1, _ptr(self._bases), _ptr(self._quals),
@@ -537,29 +512,11 @@ class MirrorPolisher:
         are uploaded once and the aligner (and later the consensus) name their inputs instead of copying them."""
         self = cls.__new__(cls)
         self.lib = load()
-        L = self.lib
-        vp = C.c_void_p
-        L.rp_mirror_polisher_open_files.restype = vp
-        L.rp_mirror_polisher_open_files.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.c_uint32, C.c_double,
-                                                    C.c_double, C.c_int, C.c_int8, C.c_int8, C.c_int8, C.c_uint32, C.c_int,
-                                                    vp, C.c_uint32]
-        L.rp_mirror_polisher_counts.restype = None
-        L.rp_mirror_polisher_counts.argtypes = [vp, vp]
-        L.rp_mirror_polisher_export.restype = None
-        L.rp_mirror_polisher_export.argtypes = [vp] * 11
-        L.rp_mirror_polisher_polish.restype = C.c_uint32
-        L.rp_mirror_polisher_polish.argtypes = [vp, C.c_int]
-        L.rp_mirror_polisher_window_consensus.restype = C.c_uint32
-        L.rp_mirror_polisher_window_consensus.argtypes = [vp, C.c_uint32, vp, C.c_uint32]
-        L.rp_mirror_polisher_polished.restype = C.c_uint64
-        L.rp_mirror_polisher_polished.argtypes = [vp, C.c_uint32, vp, vp, C.c_uint32, vp, C.c_uint64]
-        L.rp_mirror_polisher_close.restype = None
-        L.rp_mirror_polisher_close.argtypes = [vp]
         err = C.create_string_buffer(1024)
-        self.h = L.rp_mirror_polisher_open_files(os.fsencode(reads), os.fsencode(overlaps), os.fsencode(targets),
-                                                 1 if fragment_correction else 0, window_length, quality_threshold,
-                                                 error_threshold, 1 if trim else 0, match, mismatch, gap, device,
-                                                 1 if resident_reads else 0, err, 1024)
+        self.h = self.lib.rp_mirror_polisher_open_files(os.fsencode(reads), os.fsencode(overlaps), os.fsencode(targets),
+                                                        1 if fragment_correction else 0, window_length, quality_threshold,
+                                                        error_threshold, 1 if trim else 0, match, mismatch, gap, device,
+                                                        1 if resident_reads else 0, err, 1024)
         if not self.h:
             raise RuntimeError(err.value.decode(errors="replace"))
         return self
@@ -600,18 +557,13 @@ class MirrorPolisher:
         moment its last window is collected (polisher.cpp:504-537 + main.cpp:159-161).  names: target names by id
         (None: the names of the files a from_files() polisher was opened on).  resident_reads: every sequence is
         uploaded once and the windows are added by reference (layers extracted on the device)."""
-        f = self.lib.rp_mirror_polisher_stream_fasta
-        f.restype = C.c_uint32
-        f.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_char_p, C.c_uint64, C.c_int, C.c_int]
         blob = None if names is None else b"".join(n.encode() + b"\0" for n in names) + b"\0"
-        return f(self.h, 1 if drop_unpolished else 0, os.fsencode(path), blob, mem_bytes, 1 if banded else 0,
-                 1 if resident_reads else 0)
+        return self.lib.rp_mirror_polisher_stream_fasta(self.h, 1 if drop_unpolished else 0, os.fsencode(path), blob,
+                                                        mem_bytes, 1 if banded else 0, 1 if resident_reads else 0)
 
     def failed(self):
         """(overlaps, windows) the device could not finish (see host_mirror.hpp: Polisher::failed_overlaps/windows)."""
         a = (C.c_uint64 * 2)()
-        self.lib.rp_mirror_polisher_failed.restype = None
-        self.lib.rp_mirror_polisher_failed.argtypes = [C.c_void_p, C.c_void_p]
         self.lib.rp_mirror_polisher_failed(self.h, a)
         return int(a[0]), int(a[1])
 
@@ -688,17 +640,6 @@ class InputFiles:
     def __init__(self, reads, overlaps, targets, fragment_correction=False, error_threshold=0.3):
         self.lib = load()
         L = self.lib
-        vp = C.c_void_p
-        L.rp_mirror_input_open.restype = vp
-        L.rp_mirror_input_open.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.c_double, vp, C.c_uint32]
-        L.rp_mirror_input_counts.restype = None
-        L.rp_mirror_input_counts.argtypes = [vp, vp]
-        L.rp_mirror_input_export.restype = None
-        L.rp_mirror_input_export.argtypes = [vp] * 8
-        L.rp_mirror_input_cigar_breaking_points.restype = C.c_uint32
-        L.rp_mirror_input_cigar_breaking_points.argtypes = [vp, C.c_uint32, C.c_uint32, vp, C.c_uint32]
-        L.rp_mirror_input_close.restype = None
-        L.rp_mirror_input_close.argtypes = [vp]
         err = C.create_string_buffer(1024)
         self.h = L.rp_mirror_input_open(os.fsencode(reads), os.fsencode(overlaps), os.fsencode(targets),
                                         1 if fragment_correction else 0, float(error_threshold), err, 1024)

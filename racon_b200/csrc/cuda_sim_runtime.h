@@ -49,6 +49,13 @@ inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
     p->totalGlobalMem = size_t(8) << 30;
     return cudaSuccess;
 }
+enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount = 16 };
+inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr, int device) {
+    cudaDeviceProp p;
+    cudaGetDeviceProperties(&p, device);
+    *v = p.multiProcessorCount;
+    return cudaSuccess;
+}
 inline cudaError_t cudaMemGetInfo(size_t* free_b, size_t* total_b) {
     const char* e = std::getenv("RP_SIM_FREE_MB");
     *total_b = size_t(8) << 30;

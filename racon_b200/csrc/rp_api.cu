@@ -53,10 +53,20 @@ void* pinned_alloc(size_t n) {
 void pinned_free(void* p) { cudaFreeHost(p); }
 const rp::HostAllocator kPinned{pinned_alloc, pinned_free};
 
-/* growable device buffer */
+/* growable pinned host buffer: the staging of a batch object's inputs and results */
+template <typename T>
+struct PinnedBuf : rp::GrowBuf<T> {
+    PinnedBuf() : rp::GrowBuf<T>(&kPinned) {}
+};
+
+/* growable device buffer; frees its memory when destroyed */
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
     cudaError_t reserve(size_t n) {
         if (n <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -73,6 +83,72 @@ struct DevBuf {
         cap = 0;
     }
 };
+
+/* Reserves `bytes` of d and binds its memory to the kernel parameter `out`. */
+template <typename T>
+cudaError_t reserve(DevBuf& d, size_t bytes, T*& out) {
+    const cudaError_t e = d.reserve(bytes);
+    out = static_cast<T*>(d.p);
+    return e;
+}
+
+/* Copies a staged array into d (at least 16 bytes are reserved, also for an empty one) on the object's stream, adds its
+ * bytes to the object's H2D count and binds d to the kernel parameter `out`. */
+template <typename Obj, typename T>
+cudaError_t upload(Obj* o, DevBuf& d, const rp::GrowBuf<T>& h, const T*& out) {
+    const size_t bytes = h.bytes();
+    cudaError_t e = reserve(d, bytes ? bytes : 16, out);
+    if (e != cudaSuccess) return e;
+    o->last_h2d += bytes;
+    return bytes ? cudaMemcpyAsync(d.p, h.data, bytes, cudaMemcpyHostToDevice, o->stream) : cudaSuccess;
+}
+
+/* the device checks of every rp_*_create; makes the device current */
+rp_status check_device(int device) {
+    int ndev = rp_device_count();
+    if (ndev <= 0) return fail(RP_ERR_NO_DEVICE, "no CUDA device");
+    if (device < 0 || device >= ndev) return fail(RP_ERR_INVALID, "device index out of range");
+    RP_CUDA(cudaSetDevice(device));
+    return RP_OK;
+}
+
+/* The device of a batch object and the stream its work is queued on: a stream of its own, created with the object and
+ * destroyed with it, until rp_*_set_stream hands it one of the caller's. */
+struct StreamOwner {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    bool own_stream = true;
+    ~StreamOwner() {
+        if (own_stream && stream) cudaStreamDestroy(stream);
+    }
+};
+
+/* a new batch object on `device`, with a stream of its own */
+template <typename Obj>
+rp_status create_object(Obj*& o, int device) {
+    const rp_status s = check_device(device);
+    if (s != RP_OK) return s;
+    o = new (std::nothrow) Obj();
+    if (!o) return fail(RP_ERR_NOMEM, "host allocation failed");
+    o->device = device;
+    const cudaError_t e = cudaStreamCreateWithFlags(&o->stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) return RP_OK;
+    o->stream = nullptr;
+    delete o;
+    o = nullptr;
+    return fail(RP_ERR_CUDA, std::string("cudaStreamCreate: ") + cudaGetErrorString(e));
+}
+
+rp_status set_stream(StreamOwner* o, void* cuda_stream) {
+    if (!o) return fail(RP_ERR_INVALID, "null object");
+    if (o->own_stream && o->stream) {
+        cudaStreamSynchronize(o->stream);
+        cudaStreamDestroy(o->stream);
+    }
+    o->stream = static_cast<cudaStream_t>(cuda_stream);
+    o->own_stream = false;
+    return RP_OK;
+}
 
 constexpr int kWarpsPerBlock = 4;
 constexpr uint32_t kBandPaysFromWindowLength = 768;   // rows of two or more 512-column chunks
@@ -133,7 +209,6 @@ struct SimAlnJob {
         rp::aln_pair(*j->P, j->pair, j->slot);
     }
 };
-template <int kBlocksPerSm>
 void rp_aln_kernel(rp::AlnParams P, SimLaunch L) {
     const uint32_t workers = L.blocks * (L.threads / 32);
     for (;;) {
@@ -142,6 +217,12 @@ void rp_aln_kernel(rp::AlnParams P, SimLaunch L) {
         SimAlnJob job{&P, P.queue[q], P.scratch + static_cast<uint64_t>(q % workers) * P.lay.bytes};
         rp::sim::run_warp(SimAlnJob::entry, &job);
     }
+}
+template <typename Params>
+cudaError_t launch(void (*kernel)(Params, SimLaunch), uint32_t blocks, uint32_t threads, uint32_t, cudaStream_t,
+                   const Params& P) {
+    kernel(P, SimLaunch{blocks, threads});
+    return cudaSuccess;
 }
 #else
 template <int G, int KB, int kBlocksPerSm>
@@ -209,15 +290,9 @@ __global__ void __launch_bounds__(256) rp_gather_kernel(rp::GatherParams P) {
     for (uint32_t s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); s < P.n_seqs; s += warps)
         rp::gather_sequence(P, s);
 }
-/* its grid: one warp per sequence, at most 8 blocks per SM of the device */
-uint32_t gather_blocks(int device, uint32_t n_seqs) {
-    int sms = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms < 1) sms = 1;
-    return std::max<uint32_t>(1, std::min<uint32_t>(static_cast<uint32_t>(sms) * 8, (n_seqs + 7) / 8));
-}
 
-template <int kBlocksPerSm>
-__global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSm) rp_aln_kernel(rp::AlnParams P) {
+/* 4 blocks of 4 warps per SM */
+__global__ void __launch_bounds__(kWarpsPerBlock * 32, 4) rp_aln_kernel(rp::AlnParams P) {
     const int warp = threadIdx.x >> 5;
     const uint32_t worker = blockIdx.x * (blockDim.x >> 5) + warp;
     uint8_t* slot = P.scratch + static_cast<uint64_t>(worker) * P.lay.bytes;
@@ -229,7 +304,21 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSm) rp_aln_kern
         rp::aln_pair(P, P.queue[q], slot);
     }
 }
+
+template <typename Params>
+cudaError_t launch(void (*kernel)(Params), uint32_t blocks, uint32_t threads, uint32_t smem, cudaStream_t stream,
+                   const Params& P) {
+    kernel<<<blocks, threads, smem, stream>>>(P);
+    return cudaGetLastError();
+}
 #endif
+
+/* the layer-extraction grid: one warp per sequence, at most 8 blocks per SM of the device */
+uint32_t gather_blocks(int device, uint32_t n_seqs) {
+    int sms = 0;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms < 1) sms = 1;
+    return std::max<uint32_t>(1, std::min<uint32_t>(static_cast<uint32_t>(sms) * 8, (n_seqs + 7) / 8));
+}
 
 }  // namespace
 
@@ -244,13 +333,27 @@ struct rp_reads {
     bool any_quality = false;
 };
 
-struct rp_aln {
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    bool own_stream = true;
+/* Layer extraction on `stream`: packed sequence s of the batch = the store's bytes from src_pos[s] on, written to bases
+ * (and, unless weights is null, its weights from the store's qualities). */
+static cudaError_t launch_gather(const rp_reads* reads, void* bases, void* weights, const uint32_t* seq_off,
+                                 const uint64_t* src_pos, const uint8_t* src_flags, size_t n, cudaStream_t stream,
+                                 int device) {
+    rp::GatherParams G;
+    G.store_bases = static_cast<const uint8_t*>(reads->d_bases.p);
+    G.store_quals = weights ? static_cast<const uint8_t*>(reads->d_quals.p) : nullptr;
+    G.bases = static_cast<uint8_t*>(bases);
+    G.weights = static_cast<uint8_t*>(weights);
+    G.seq_off = seq_off;
+    G.src_pos = src_pos;
+    G.src_flags = src_flags;
+    G.n_seqs = static_cast<uint32_t>(n);
+    return launch(rp_gather_kernel, gather_blocks(device, G.n_seqs), 256, 0, stream, G);
+}
+
+struct rp_aln : StreamOwner {
     rp::AlnParams P;
-    rp::GrowBuf<uint8_t> bases;
-    rp::GrowBuf<uint32_t> q_off, q_len, t_off, t_len, run_off, run_cap, queue, t_begin, q_start, bp_off, bp_cap;
+    PinnedBuf<uint8_t> bases;
+    PinnedBuf<uint32_t> q_off, q_len, t_off, t_len, run_off, run_cap, queue, t_begin, q_start, bp_off, bp_cap;
     uint32_t window_length = 0;
     uint64_t bp_total = 0;
     std::vector<uint32_t> pre_status;      // per pair: soft status decided on the host (too long) or 0
@@ -259,45 +362,35 @@ struct rp_aln {
     const rp_reads* reads = nullptr;
     bool by_ref = false;
     uint64_t n_bases = 0;              // == bases.size unless by_ref
-    rp::GrowBuf<uint64_t> src_pos;     // two entries per pair: query, target
-    rp::GrowBuf<uint8_t> src_flags;
-    rp::GrowBuf<uint32_t> span_off;    // packed offsets of the 2 n spans, + total
+    PinnedBuf<uint64_t> src_pos;     // two entries per pair: query, target
+    PinnedBuf<uint8_t> src_flags;
+    PinnedBuf<uint32_t> span_off;    // packed offsets of the 2 n spans, + total
     DevBuf d_src_pos, d_src_flags, d_span_off;
     DevBuf d_bases, d_q_off, d_q_len, d_t_off, d_t_len, d_run_off, d_run_cap, d_queue, d_runs, d_n_runs, d_dist,
         d_status, d_head, d_scratch, d_t_begin, d_q_start, d_bp_off, d_bp_cap, d_bp, d_n_bp;
-    rp::GrowBuf<uint32_t> h_runs, h_n_runs, h_status, h_bp, h_n_bp;
-    rp::GrowBuf<int32_t> h_dist;
+    PinnedBuf<uint32_t> h_runs, h_n_runs, h_status, h_bp, h_n_bp;
+    PinnedBuf<int32_t> h_dist;
     std::vector<std::string> cigars;
     std::vector<uint8_t> cigar_built;
     uint32_t workers = 0;
     int grid = 0;
-    int blocks_per_sm = 4;
     uint32_t max_len = 0;
     uint64_t max_bases = 0;
     bool uploaded = false, launched = false, downloaded = false, synced = false;
     uint64_t launches = 0, last_h2d = 0, last_d2h = 0;
-    rp_aln()
-        : bases(&kPinned), q_off(&kPinned), q_len(&kPinned), t_off(&kPinned), t_len(&kPinned), run_off(&kPinned),
-          run_cap(&kPinned), queue(&kPinned), t_begin(&kPinned), q_start(&kPinned), bp_off(&kPinned),
-          bp_cap(&kPinned), src_pos(&kPinned), src_flags(&kPinned), span_off(&kPinned), h_runs(&kPinned),
-          h_n_runs(&kPinned), h_status(&kPinned), h_bp(&kPinned), h_n_bp(&kPinned), h_dist(&kPinned) {
-        std::memset(&P, 0, sizeof(P));
-    }
+    rp_aln() { std::memset(&P, 0, sizeof(P)); }
 };
 
-struct rp_poa {
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    bool own_stream = true;
-    rp::PackedBatch batch;
+struct rp_poa : StreamOwner {
+    rp::PackedBatch batch{&kPinned};
     rp::PoaParams P;
     /* device input buffers */
     DevBuf d_bases, d_weights, d_seq_flags, d_win_flags, d_seq_off, d_seq_begin, d_seq_end, d_win_first, d_out_off,
         d_out_cap, d_queue, d_win_alpha, d_cons, d_cov, d_len, d_status, d_head, d_stats, d_scratch;
     /* pinned results */
-    rp::GrowBuf<uint8_t> h_cons;
-    rp::GrowBuf<uint16_t> h_cov;
-    rp::GrowBuf<uint32_t> h_len, h_status;
+    PinnedBuf<uint8_t> h_cons;
+    PinnedBuf<uint16_t> h_cov;
+    PinnedBuf<uint32_t> h_len, h_status;
     uint64_t h_stats[8] = {0};
     uint32_t workers = 0;          // lane groups = windows in flight
     int grid = 0;
@@ -327,9 +420,7 @@ struct rp_poa {
     uint64_t escalated = 0;
     size_t mem_budget = 0;
 
-    rp_poa() : batch(&kPinned), h_cons(&kPinned), h_cov(&kPinned), h_len(&kPinned), h_status(&kPinned) {
-        std::memset(&P, 0, sizeof(P));
-    }
+    rp_poa() { std::memset(&P, 0, sizeof(P)); }
 };
 
 extern "C" {
@@ -366,19 +457,10 @@ rp_status rp_poa_create(rp_poa** out, int device, size_t mem_bytes, int8_t match
     if (!out) return fail(RP_ERR_INVALID, "null out");
     *out = nullptr;
     if (gap > 0) return fail(RP_ERR_INVALID, "gap penalty must be non-positive (alignment_engine.cpp:47-51)");
-    int ndev = rp_device_count();
-    if (ndev <= 0) return fail(RP_ERR_NO_DEVICE, "no CUDA device");
-    if (device < 0 || device >= ndev) return fail(RP_ERR_INVALID, "device index out of range");
-    RP_CUDA(cudaSetDevice(device));
-    rp_poa* p = new (std::nothrow) rp_poa();
-    if (!p) return fail(RP_ERR_NOMEM, "host allocation failed");
-    p->device = device;
+    rp_poa* p = nullptr;
+    const rp_status st = create_object(p, device);
+    if (st != RP_OK) return st;
     p->banded = banded;
-    cudaError_t e = cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) {
-        delete p;
-        return fail(RP_ERR_CUDA, std::string("cudaStreamCreate: ") + cudaGetErrorString(e));
-    }
     rp::set_scores(p->P, match, mismatch, gap);
     p->P.banded = banded ? 1 : 0;   // the request; configure() decides whether the band layout is used (window length)
     size_t free_b = 0, total_b = 0;
@@ -391,7 +473,7 @@ rp_status rp_poa_create(rp_poa** out, int device, size_t mem_bytes, int8_t match
     p->batch.max_bases = std::min<uint64_t>(0xfff00000ull, std::max<uint64_t>(io_budget / 4, 1u << 16));
     p->batch.max_out = std::min<uint64_t>(0xfff00000ull, std::max<uint64_t>(io_budget / 8, 1u << 14));
     p->batch.max_windows = static_cast<uint32_t>(std::min<uint64_t>(1u << 22, std::max<uint64_t>(io_budget / 4096, 16)));
-    e = p->d_head.reserve(256);
+    cudaError_t e = p->d_head.reserve(256);
     if (e == cudaSuccess) e = p->d_stats.reserve(256);
     if (e != cudaSuccess) {
         rp_poa_destroy(p);
@@ -533,25 +615,10 @@ void rp_poa_destroy(rp_poa* p) {
                         "band alignments differ from the full-matrix alignment (audit)\n",
                 static_cast<unsigned>(p->group * p->band_k), static_cast<unsigned long long>(p->band_total[0]),
                 static_cast<unsigned long long>(p->band_total[1]), static_cast<unsigned long long>(p->band_total[2]));
-    DevBuf* bufs[] = {&p->d_bases, &p->d_weights, &p->d_seq_flags, &p->d_win_flags, &p->d_seq_off, &p->d_seq_begin,
-                      &p->d_seq_end, &p->d_win_first, &p->d_out_off, &p->d_out_cap, &p->d_queue, &p->d_win_alpha,
-                      &p->d_cons, &p->d_cov, &p->d_len, &p->d_status, &p->d_head, &p->d_stats, &p->d_scratch,
-                      &p->d_scratch_big, &p->d_queue_big, &p->d_src_pos, &p->d_src_flags};
-    for (DevBuf* b : bufs) b->release();
-    if (p->own_stream && p->stream) cudaStreamDestroy(p->stream);
-    delete p;
+    delete p;   // frees the device buffers, then destroys the object's own stream
 }
 
-rp_status rp_poa_set_stream(rp_poa* p, void* cuda_stream) {
-    if (!p) return fail(RP_ERR_INVALID, "null object");
-    if (p->own_stream && p->stream) {
-        cudaStreamSynchronize(p->stream);
-        cudaStreamDestroy(p->stream);
-    }
-    p->stream = static_cast<cudaStream_t>(cuda_stream);
-    p->own_stream = false;
-    return RP_OK;
-}
+rp_status rp_poa_set_stream(rp_poa* p, void* cuda_stream) { return set_stream(p, cuda_stream); }
 
 static rp_status map_pack(int r) {
     switch (r) {
@@ -576,10 +643,8 @@ rp_status rp_reads_create(rp_reads** out, int device, uint32_t n_seqs, const cha
     if (!out) return fail(RP_ERR_INVALID, "null out");
     *out = nullptr;
     if (!data || !length) return fail(RP_ERR_INVALID, "null argument");
-    int ndev = rp_device_count();
-    if (ndev <= 0) return fail(RP_ERR_NO_DEVICE, "no CUDA device");
-    if (device < 0 || device >= ndev) return fail(RP_ERR_INVALID, "device index out of range");
-    RP_CUDA(cudaSetDevice(device));
+    const rp_status s = check_device(device);
+    if (s != RP_OK) return s;
     rp_reads* r = new (std::nothrow) rp_reads();
     if (!r) return fail(RP_ERR_NOMEM, "host allocation failed");
     r->device = device;
@@ -617,8 +682,6 @@ rp_status rp_reads_create(rp_reads** out, int device, uint32_t n_seqs, const cha
     if (e == cudaSuccess) e = cudaHostAlloc(&stage, stage_bytes, cudaHostAllocDefault);
     if (e != cudaSuccess) {
         cudaGetLastError();
-        r->d_bases.release();
-        r->d_quals.release();
         delete r;
         return fail(RP_ERR_NOMEM, std::string("read store allocation: ") + cudaGetErrorString(e));
     }
@@ -655,8 +718,6 @@ rp_status rp_reads_create(rp_reads** out, int device, uint32_t n_seqs, const cha
     if (st) cudaStreamDestroy(st);
     cudaFreeHost(stage);
     if (e != cudaSuccess) {
-        r->d_bases.release();
-        r->d_quals.release();
         delete r;
         return fail(RP_ERR_CUDA, std::string("read store upload: ") + cudaGetErrorString(e));
     }
@@ -667,8 +728,6 @@ rp_status rp_reads_create(rp_reads** out, int device, uint32_t n_seqs, const cha
 void rp_reads_destroy(rp_reads* r) {
     if (!r) return;
     cudaSetDevice(r->device);
-    r->d_bases.release();
-    r->d_quals.release();
     delete r;
 }
 
@@ -859,81 +918,47 @@ rp_status rp_poa_upload(rp_poa* p) {
         rp_status cs = configure(p, wl);
         if (cs != RP_OK) return cs;
     }
-    uint64_t h2d = 0;
-    auto up = [&](DevBuf& d, const void* src, size_t bytes) -> cudaError_t {
-        cudaError_t e = d.reserve(bytes ? bytes : 16);
-        if (e != cudaSuccess) return e;
-        h2d += bytes;
-        return bytes ? cudaMemcpyAsync(d.p, src, bytes, cudaMemcpyHostToDevice, p->stream) : cudaSuccess;
-    };
+    rp::PoaParams& P = p->P;
+    const uint64_t* src_pos = nullptr;
+    const uint8_t* src_flags = nullptr;
+    p->last_h2d = 0;
     if (b.by_ref) {
-        RP_CUDA(p->d_bases.reserve(b.n_bases + 16));
-        RP_CUDA(p->d_weights.reserve(b.n_bases + 16));
-        RP_CUDA(up(p->d_src_pos, b.src_pos.data, b.src_pos.bytes()));
-        RP_CUDA(up(p->d_src_flags, b.src_flags.data, b.src_flags.bytes()));
+        RP_CUDA(reserve(p->d_bases, b.n_bases + 16, P.bases));
+        RP_CUDA(reserve(p->d_weights, b.n_bases + 16, P.weights));
+        RP_CUDA(upload(p, p->d_src_pos, b.src_pos, src_pos));
+        RP_CUDA(upload(p, p->d_src_flags, b.src_flags, src_flags));
     } else {
-        RP_CUDA(up(p->d_bases, b.bases.data, b.bases.bytes()));
-        RP_CUDA(up(p->d_weights, b.weights.data, b.weights.bytes()));
+        RP_CUDA(upload(p, p->d_bases, b.bases, P.bases));
+        RP_CUDA(upload(p, p->d_weights, b.weights, P.weights));
     }
-    RP_CUDA(up(p->d_seq_off, b.seq_off.data, b.seq_off.bytes()));
-    RP_CUDA(up(p->d_seq_begin, b.seq_begin.data, b.seq_begin.bytes()));
-    RP_CUDA(up(p->d_seq_end, b.seq_end.data, b.seq_end.bytes()));
-    RP_CUDA(up(p->d_seq_flags, b.seq_flags.data, b.seq_flags.bytes()));
-    RP_CUDA(up(p->d_win_first, b.win_first.data, b.win_first.bytes()));
-    RP_CUDA(up(p->d_win_flags, b.win_flags.data, b.win_flags.bytes()));
-    RP_CUDA(up(p->d_win_alpha, b.win_alpha.data, b.win_alpha.bytes()));
-    RP_CUDA(up(p->d_out_off, b.out_off.data, b.out_off.bytes()));
-    RP_CUDA(up(p->d_out_cap, b.out_cap.data, b.out_cap.bytes()));
-    RP_CUDA(up(p->d_queue, b.queue.data, b.queue.bytes()));
-    RP_CUDA(p->d_cons.reserve(b.out_total + 16));
-    RP_CUDA(p->d_cov.reserve((b.out_total + 16) * 2));
-    RP_CUDA(p->d_len.reserve((n + 1) * 4));
-    RP_CUDA(p->d_status.reserve((n + 1) * 4));
+    RP_CUDA(upload(p, p->d_seq_off, b.seq_off, P.seq_off));
+    RP_CUDA(upload(p, p->d_seq_begin, b.seq_begin, P.seq_begin));
+    RP_CUDA(upload(p, p->d_seq_end, b.seq_end, P.seq_end));
+    RP_CUDA(upload(p, p->d_seq_flags, b.seq_flags, P.seq_flags));
+    RP_CUDA(upload(p, p->d_win_first, b.win_first, P.win_first));
+    RP_CUDA(upload(p, p->d_win_flags, b.win_flags, P.win_flags));
+    RP_CUDA(upload(p, p->d_win_alpha, b.win_alpha, P.win_alpha));
+    RP_CUDA(upload(p, p->d_out_off, b.out_off, P.out_off));
+    RP_CUDA(upload(p, p->d_out_cap, b.out_cap, P.out_cap));
+    RP_CUDA(upload(p, p->d_queue, b.queue, P.queue));
+    RP_CUDA(reserve(p->d_cons, b.out_total + 16, P.cons));
+    RP_CUDA(reserve(p->d_cov, (b.out_total + 16) * 2, P.cons_cov));
+    RP_CUDA(reserve(p->d_len, (n + 1) * 4, P.cons_len));
+    RP_CUDA(reserve(p->d_status, (n + 1) * 4, P.status));
     if (!p->h_cons.reserve(b.out_total + 16) || !p->h_cov.reserve(b.out_total + 16) || !p->h_len.reserve(n + 1) ||
         !p->h_status.reserve(n + 1))
         return fail(RP_ERR_NOMEM, "pinned result allocation failed");
-    rp::PoaParams& P = p->P;
     P.n_windows = n;
-    P.bases = static_cast<const uint8_t*>(p->d_bases.p);
-    P.weights = static_cast<const uint8_t*>(p->d_weights.p);
-    P.seq_off = static_cast<const uint32_t*>(p->d_seq_off.p);
-    P.seq_begin = static_cast<const uint32_t*>(p->d_seq_begin.p);
-    P.seq_end = static_cast<const uint32_t*>(p->d_seq_end.p);
-    P.seq_flags = static_cast<const uint8_t*>(p->d_seq_flags.p);
-    P.win_first = static_cast<const uint32_t*>(p->d_win_first.p);
-    P.win_flags = static_cast<const uint8_t*>(p->d_win_flags.p);
-    P.win_alpha = static_cast<const uint64_t*>(p->d_win_alpha.p);
-    P.queue = static_cast<const uint32_t*>(p->d_queue.p);
     P.queue_head = static_cast<uint32_t*>(p->d_head.p);
-    P.cons = static_cast<uint8_t*>(p->d_cons.p);
-    P.cons_cov = static_cast<uint16_t*>(p->d_cov.p);
-    P.out_off = static_cast<const uint32_t*>(p->d_out_off.p);
-    P.out_cap = static_cast<const uint32_t*>(p->d_out_cap.p);
-    P.cons_len = static_cast<uint32_t*>(p->d_len.p);
-    P.status = static_cast<uint32_t*>(p->d_status.p);
     P.stats = p->counters ? static_cast<uint64_t*>(p->d_stats.p) : nullptr;
     P.scratch = static_cast<uint8_t*>(p->d_scratch.p);
     if (b.by_ref && b.src_pos.size > 0) {
         /* layer extraction on the device: fills d_bases / d_weights from the store, on this object's stream, ahead of the
          * POA kernel */
-        rp::GatherParams G;
-        G.store_bases = static_cast<const uint8_t*>(p->reads->d_bases.p);
-        G.store_quals = static_cast<const uint8_t*>(p->reads->d_quals.p);
-        G.bases = static_cast<uint8_t*>(p->d_bases.p);
-        G.weights = static_cast<uint8_t*>(p->d_weights.p);
-        G.seq_off = P.seq_off;
-        G.src_pos = static_cast<const uint64_t*>(p->d_src_pos.p);
-        G.src_flags = static_cast<const uint8_t*>(p->d_src_flags.p);
-        G.n_seqs = static_cast<uint32_t>(b.src_pos.size);
-#if defined(RP_HOST_SIM)
-        rp_gather_kernel(G, SimLaunch{1, 256});
-#else
-        rp_gather_kernel<<<gather_blocks(p->device, G.n_seqs), 256, 0, p->stream>>>(G);
-        RP_CUDA(cudaGetLastError());
-#endif
+        RP_CUDA(launch_gather(p->reads, p->d_bases.p, p->d_weights.p, P.seq_off, src_pos, src_flags, b.src_pos.size,
+                              p->stream, p->device));
         p->gather_launches += 1;
     }
-    p->last_h2d = h2d;
     p->uploaded = true;
     p->launched = p->downloaded = p->synced = false;
     return RP_OK;
@@ -950,16 +975,21 @@ rp_status rp_poa_launch(rp_poa* p) {
         p->P.band_stats = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(p->d_stats.p) + 128);
         const uint32_t need_blocks = (p->P.n_windows + p->groups_per_block - 1) / p->groups_per_block;
         const uint32_t blocks = std::min<uint32_t>(static_cast<uint32_t>(p->grid), need_blocks);
-#if defined(RP_HOST_SIM)
-        p->kernel(p->P, SimLaunch{blocks, kWarpsPerBlock * 32});
-#else
-        p->kernel<<<blocks, kWarpsPerBlock * 32, p->smem_block, p->stream>>>(p->P);
-#endif
-        RP_CUDA(cudaGetLastError());
+        RP_CUDA(launch(p->kernel, blocks, kWarpsPerBlock * 32, p->smem_block, p->stream, p->P));
         p->launches += 1;
     }
     p->launched = true;
     p->downloaded = p->synced = false;
+    return RP_OK;
+}
+
+/* queues the copies of the results of the batch's n GPU windows (consensus, coverage, lengths, statuses) to pinned memory */
+static rp_status read_results(rp_poa* p, uint32_t n) {
+    const size_t tot = p->batch.out_total;
+    RP_CUDA(cudaMemcpyAsync(p->h_cons.data, p->d_cons.p, tot, cudaMemcpyDeviceToHost, p->stream));
+    RP_CUDA(cudaMemcpyAsync(p->h_cov.data, p->d_cov.p, tot * 2, cudaMemcpyDeviceToHost, p->stream));
+    RP_CUDA(cudaMemcpyAsync(p->h_len.data, p->d_len.p, n * 4, cudaMemcpyDeviceToHost, p->stream));
+    RP_CUDA(cudaMemcpyAsync(p->h_status.data, p->d_status.p, n * 4, cudaMemcpyDeviceToHost, p->stream));
     return RP_OK;
 }
 
@@ -970,12 +1000,9 @@ rp_status rp_poa_download(rp_poa* p) {
     const uint32_t n = p->P.n_windows;
     uint64_t d2h = 0;
     if (n > 0) {
-        size_t tot = p->batch.out_total;
-        RP_CUDA(cudaMemcpyAsync(p->h_cons.data, p->d_cons.p, tot, cudaMemcpyDeviceToHost, p->stream));
-        RP_CUDA(cudaMemcpyAsync(p->h_cov.data, p->d_cov.p, tot * 2, cudaMemcpyDeviceToHost, p->stream));
-        RP_CUDA(cudaMemcpyAsync(p->h_len.data, p->d_len.p, n * 4, cudaMemcpyDeviceToHost, p->stream));
-        RP_CUDA(cudaMemcpyAsync(p->h_status.data, p->d_status.p, n * 4, cudaMemcpyDeviceToHost, p->stream));
-        d2h = tot * 3 + static_cast<uint64_t>(n) * 8;
+        const rp_status s = read_results(p, n);
+        if (s != RP_OK) return s;
+        d2h = p->batch.out_total * 3 + static_cast<uint64_t>(n) * 8;
     }
     if (p->counters)
         RP_CUDA(cudaMemcpyAsync(p->h_stats, p->d_stats.p, 64, cudaMemcpyDeviceToHost, p->stream));
@@ -1037,19 +1064,11 @@ static rp_status escalate(rp_poa* p) {
     P.band_stats = nullptr;
     uint32_t blocks = std::min<uint32_t>(p->workers_big / p->groups_per_block,
                                          (static_cast<uint32_t>(redo.size()) + p->groups_per_block - 1) / p->groups_per_block);
-#if defined(RP_HOST_SIM)
-    p->kernel(P, SimLaunch{blocks, kWarpsPerBlock * 32});
-#else
-    p->kernel<<<blocks, kWarpsPerBlock * 32, p->smem_block, p->stream>>>(P);
-#endif
-    RP_CUDA(cudaGetLastError());
+    RP_CUDA(launch(p->kernel, blocks, kWarpsPerBlock * 32, p->smem_block, p->stream, P));
     p->launches += 1;
     p->escalated += redo.size();
-    size_t tot = p->batch.out_total;
-    RP_CUDA(cudaMemcpyAsync(p->h_cons.data, p->d_cons.p, tot, cudaMemcpyDeviceToHost, p->stream));
-    RP_CUDA(cudaMemcpyAsync(p->h_cov.data, p->d_cov.p, tot * 2, cudaMemcpyDeviceToHost, p->stream));
-    RP_CUDA(cudaMemcpyAsync(p->h_len.data, p->d_len.p, n * 4, cudaMemcpyDeviceToHost, p->stream));
-    RP_CUDA(cudaMemcpyAsync(p->h_status.data, p->d_status.p, n * 4, cudaMemcpyDeviceToHost, p->stream));
+    const rp_status s = read_results(p, n);
+    if (s != RP_OK) return s;
     RP_CUDA(cudaStreamSynchronize(p->stream));
     return RP_OK;
 }
@@ -1181,18 +1200,9 @@ rp_status rp_poa_enable_counters(rp_poa* p, int on) {
 rp_status rp_aln_create(rp_aln** out, int device, size_t mem_bytes, uint32_t max_len) {
     if (!out) return fail(RP_ERR_INVALID, "null out");
     *out = nullptr;
-    int ndev = rp_device_count();
-    if (ndev <= 0) return fail(RP_ERR_NO_DEVICE, "no CUDA device");
-    if (device < 0 || device >= ndev) return fail(RP_ERR_INVALID, "device index out of range");
-    RP_CUDA(cudaSetDevice(device));
-    rp_aln* a = new (std::nothrow) rp_aln();
-    if (!a) return fail(RP_ERR_NOMEM, "host allocation failed");
-    a->device = device;
-    cudaError_t e = cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) {
-        delete a;
-        return fail(RP_ERR_CUDA, std::string("cudaStreamCreate: ") + cudaGetErrorString(e));
-    }
+    rp_aln* a = nullptr;
+    const rp_status st = create_object(a, device);
+    if (st != RP_OK) return st;
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
     size_t free_b = 0, total_b = 0;
@@ -1203,16 +1213,7 @@ rp_status rp_aln_create(rp_aln** out, int device, size_t mem_bytes, uint32_t max
     a->P.lim.store_words = 53000;  // > 1 MiB / 20 B: the largest base case edlib's rule allows
     a->P.lay = rp::make_aln_layout(a->P.lim);
     int occ = 0;
-    if (const char* env = std::getenv("RP_ALN_BLOCKS_PER_SM")) {  // tuning knob (tools/bench_aln.py); default 4
-        int v = std::atoi(env);
-        if (v == 4 || v == 6 || v == 8) a->blocks_per_sm = v;
-    }
-    if (a->blocks_per_sm == 8)
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rp_aln_kernel<8>, kWarpsPerBlock * 32, 0);
-    else if (a->blocks_per_sm == 6)
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rp_aln_kernel<6>, kWarpsPerBlock * 32, 0);
-    else
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rp_aln_kernel<4>, kWarpsPerBlock * 32, 0);
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rp_aln_kernel, kWarpsPerBlock * 32, 0);
     if (e != cudaSuccess || occ < 1) {
         rp_aln_destroy(a);
         return fail(RP_ERR_CUDA, std::string("kernel configuration: ") + cudaGetErrorString(e));
@@ -1241,25 +1242,10 @@ void rp_aln_destroy(rp_aln* a) {
     if (!a) return;
     cudaSetDevice(a->device);
     if (a->stream) cudaStreamSynchronize(a->stream);
-    DevBuf* bufs[] = {&a->d_bases, &a->d_q_off, &a->d_q_len, &a->d_t_off, &a->d_t_len, &a->d_run_off, &a->d_run_cap,
-                      &a->d_queue, &a->d_runs, &a->d_n_runs, &a->d_dist, &a->d_status, &a->d_head, &a->d_scratch,
-                      &a->d_t_begin, &a->d_q_start, &a->d_bp_off, &a->d_bp_cap, &a->d_bp, &a->d_n_bp, &a->d_src_pos,
-                      &a->d_src_flags, &a->d_span_off};
-    for (DevBuf* b : bufs) b->release();
-    if (a->own_stream && a->stream) cudaStreamDestroy(a->stream);
-    delete a;
+    delete a;   // frees the device buffers, then destroys the object's own stream
 }
 
-rp_status rp_aln_set_stream(rp_aln* a, void* cuda_stream) {
-    if (!a) return fail(RP_ERR_INVALID, "null object");
-    if (a->own_stream && a->stream) {
-        cudaStreamSynchronize(a->stream);
-        cudaStreamDestroy(a->stream);
-    }
-    a->stream = static_cast<cudaStream_t>(cuda_stream);
-    a->own_stream = false;
-    return RP_OK;
-}
+rp_status rp_aln_set_stream(rp_aln* a, void* cuda_stream) { return set_stream(a, cuda_stream); }
 
 rp_status rp_aln_set_window_length(rp_aln* a, uint32_t window_length) {
     if (!a) return fail(RP_ERR_INVALID, "null object");
@@ -1361,87 +1347,51 @@ rp_status rp_aln_upload(rp_aln* a) {
     a->queue.clear();
     if (!a->queue.reserve(n ? n : 1)) return fail(RP_ERR_NOMEM, "queue allocation failed");
     for (uint32_t i = 0; i < n; ++i) a->queue.push(idx[i]);
-    uint64_t h2d = 0;
-    auto up = [&](DevBuf& d, const void* src, size_t bytes) -> cudaError_t {
-        cudaError_t e = d.reserve(bytes ? bytes : 16);
-        if (e != cudaSuccess) return e;
-        h2d += bytes;
-        return bytes ? cudaMemcpyAsync(d.p, src, bytes, cudaMemcpyHostToDevice, a->stream) : cudaSuccess;
-    };
+    rp::AlnParams& P = a->P;
+    a->last_h2d = 0;
     if (a->by_ref) {
-        RP_CUDA(a->d_bases.reserve(a->n_bases + 16));
-        RP_CUDA(up(a->d_src_pos, a->src_pos.data, a->src_pos.bytes()));
-        RP_CUDA(up(a->d_src_flags, a->src_flags.data, a->src_flags.bytes()));
-        RP_CUDA(up(a->d_span_off, a->span_off.data, a->span_off.bytes()));
+        const uint64_t* src_pos = nullptr;
+        const uint8_t* src_flags = nullptr;
+        const uint32_t* span_off = nullptr;
+        RP_CUDA(reserve(a->d_bases, a->n_bases + 16, P.bases));
+        RP_CUDA(upload(a, a->d_src_pos, a->src_pos, src_pos));
+        RP_CUDA(upload(a, a->d_src_flags, a->src_flags, src_flags));
+        RP_CUDA(upload(a, a->d_span_off, a->span_off, span_off));
         /* both spans of every pair are cut out of the store on the device (reverse complement included) */
-        rp::GatherParams G;
-        G.store_bases = static_cast<const uint8_t*>(a->reads->d_bases.p);
-        G.store_quals = nullptr;
-        G.bases = static_cast<uint8_t*>(a->d_bases.p);
-        G.weights = nullptr;
-        G.seq_off = static_cast<const uint32_t*>(a->d_span_off.p);
-        G.src_pos = static_cast<const uint64_t*>(a->d_src_pos.p);
-        G.src_flags = static_cast<const uint8_t*>(a->d_src_flags.p);
-        G.n_seqs = static_cast<uint32_t>(a->src_pos.size);
-        if (G.n_seqs > 0) {
-#if defined(RP_HOST_SIM)
-            rp_gather_kernel(G, SimLaunch{1, 256});
-#else
-            rp_gather_kernel<<<gather_blocks(a->device, G.n_seqs), 256, 0, a->stream>>>(G);
-            RP_CUDA(cudaGetLastError());
-#endif
-        }
+        if (a->src_pos.size > 0)
+            RP_CUDA(launch_gather(a->reads, a->d_bases.p, nullptr, span_off, src_pos, src_flags, a->src_pos.size,
+                                  a->stream, a->device));
     } else {
-        RP_CUDA(up(a->d_bases, a->bases.data, a->bases.bytes()));
+        RP_CUDA(upload(a, a->d_bases, a->bases, P.bases));
     }
-    RP_CUDA(up(a->d_q_off, a->q_off.data, a->q_off.bytes()));
-    RP_CUDA(up(a->d_q_len, a->q_len.data, a->q_len.bytes()));
-    RP_CUDA(up(a->d_t_off, a->t_off.data, a->t_off.bytes()));
-    RP_CUDA(up(a->d_t_len, a->t_len.data, a->t_len.bytes()));
-    RP_CUDA(up(a->d_run_off, a->run_off.data, a->run_off.bytes()));
-    RP_CUDA(up(a->d_run_cap, a->run_cap.data, a->run_cap.bytes()));
-    RP_CUDA(up(a->d_queue, a->queue.data, a->queue.bytes()));
+    RP_CUDA(upload(a, a->d_q_off, a->q_off, P.q_off));
+    RP_CUDA(upload(a, a->d_q_len, a->q_len, P.q_len));
+    RP_CUDA(upload(a, a->d_t_off, a->t_off, P.t_off));
+    RP_CUDA(upload(a, a->d_t_len, a->t_len, P.t_len));
+    RP_CUDA(upload(a, a->d_run_off, a->run_off, P.run_off));
+    RP_CUDA(upload(a, a->d_run_cap, a->run_cap, P.run_cap));
+    RP_CUDA(upload(a, a->d_queue, a->queue, P.queue));
     if (a->window_length) {
-        RP_CUDA(up(a->d_t_begin, a->t_begin.data, a->t_begin.bytes()));
-        RP_CUDA(up(a->d_q_start, a->q_start.data, a->q_start.bytes()));
-        RP_CUDA(up(a->d_bp_off, a->bp_off.data, a->bp_off.bytes()));
-        RP_CUDA(up(a->d_bp_cap, a->bp_cap.data, a->bp_cap.bytes()));
-        RP_CUDA(a->d_bp.reserve((a->bp_total + 4) * 8));
-        RP_CUDA(a->d_n_bp.reserve((n + 1) * 4));
+        RP_CUDA(upload(a, a->d_t_begin, a->t_begin, P.t_begin));
+        RP_CUDA(upload(a, a->d_q_start, a->q_start, P.q_start));
+        RP_CUDA(upload(a, a->d_bp_off, a->bp_off, P.bp_off));
+        RP_CUDA(upload(a, a->d_bp_cap, a->bp_cap, P.bp_cap));
+        RP_CUDA(reserve(a->d_bp, (a->bp_total + 4) * 8, P.bp));
+        RP_CUDA(reserve(a->d_n_bp, (n + 1) * 4, P.n_bp));
         if (!a->h_bp.reserve(2 * a->bp_total + 8) || !a->h_n_bp.reserve(n + 1))
             return fail(RP_ERR_NOMEM, "pinned result allocation failed");
     }
-    RP_CUDA(a->d_runs.reserve((a->run_total + 16) * 4));
-    RP_CUDA(a->d_n_runs.reserve((n + 1) * 4));
-    RP_CUDA(a->d_dist.reserve((n + 1) * 4));
-    RP_CUDA(a->d_status.reserve((n + 1) * 4));
+    RP_CUDA(reserve(a->d_runs, (a->run_total + 16) * 4, P.runs));
+    RP_CUDA(reserve(a->d_n_runs, (n + 1) * 4, P.n_runs));
+    RP_CUDA(reserve(a->d_dist, (n + 1) * 4, P.dist));
+    RP_CUDA(reserve(a->d_status, (n + 1) * 4, P.status));
     if (!a->h_runs.reserve(a->run_total + 16) || !a->h_n_runs.reserve(n + 1) || !a->h_status.reserve(n + 1) ||
         !a->h_dist.reserve(n + 1))
         return fail(RP_ERR_NOMEM, "pinned result allocation failed");
-    rp::AlnParams& P = a->P;
     P.n_pairs = n;
-    P.bases = static_cast<const uint8_t*>(a->d_bases.p);
-    P.q_off = static_cast<const uint32_t*>(a->d_q_off.p);
-    P.q_len = static_cast<const uint32_t*>(a->d_q_len.p);
-    P.t_off = static_cast<const uint32_t*>(a->d_t_off.p);
-    P.t_len = static_cast<const uint32_t*>(a->d_t_len.p);
-    P.queue = static_cast<const uint32_t*>(a->d_queue.p);
     P.queue_head = static_cast<uint32_t*>(a->d_head.p);
-    P.runs = static_cast<uint32_t*>(a->d_runs.p);
-    P.run_off = static_cast<const uint32_t*>(a->d_run_off.p);
-    P.run_cap = static_cast<const uint32_t*>(a->d_run_cap.p);
-    P.n_runs = static_cast<uint32_t*>(a->d_n_runs.p);
-    P.dist = static_cast<int32_t*>(a->d_dist.p);
-    P.status = static_cast<uint32_t*>(a->d_status.p);
     P.scratch = static_cast<uint8_t*>(a->d_scratch.p);
     P.window_length = a->window_length;
-    P.t_begin = static_cast<const uint32_t*>(a->d_t_begin.p);
-    P.q_start = static_cast<const uint32_t*>(a->d_q_start.p);
-    P.bp = static_cast<uint32_t*>(a->d_bp.p);
-    P.bp_off = static_cast<const uint32_t*>(a->d_bp_off.p);
-    P.bp_cap = static_cast<const uint32_t*>(a->d_bp_cap.p);
-    P.n_bp = static_cast<uint32_t*>(a->d_n_bp.p);
-    a->last_h2d = h2d;
     a->uploaded = true;
     a->launched = a->downloaded = a->synced = false;
     return RP_OK;
@@ -1453,17 +1403,7 @@ rp_status rp_aln_launch(rp_aln* a) {
     RP_CUDA(cudaSetDevice(a->device));
     if (a->P.n_pairs > 0) {
         RP_CUDA(cudaMemsetAsync(a->d_head.p, 0, 4, a->stream));
-#if defined(RP_HOST_SIM)
-        rp_aln_kernel<4>(a->P, SimLaunch{static_cast<uint32_t>(a->grid), kWarpsPerBlock * 32});
-#else
-        if (a->blocks_per_sm == 8)
-            rp_aln_kernel<8><<<a->grid, kWarpsPerBlock * 32, 0, a->stream>>>(a->P);
-        else if (a->blocks_per_sm == 6)
-            rp_aln_kernel<6><<<a->grid, kWarpsPerBlock * 32, 0, a->stream>>>(a->P);
-        else
-            rp_aln_kernel<4><<<a->grid, kWarpsPerBlock * 32, 0, a->stream>>>(a->P);
-#endif
-        RP_CUDA(cudaGetLastError());
+        RP_CUDA(launch(rp_aln_kernel, static_cast<uint32_t>(a->grid), kWarpsPerBlock * 32, 0, a->stream, a->P));
         a->launches += 1;
     }
     a->launched = true;

@@ -17,6 +17,22 @@ def declared_symbols():
     return sorted(set(re.findall(r"\b(rp_[a-z0-9_]+)\s*\(", txt)))
 
 
+def declared_parameter_counts():
+    """{symbol: number of parameters} of every prototype in include/racon_b200.h ((void) = 0)"""
+    txt = open(os.path.join(ROOT, "include", "racon_b200.h")).read()
+    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
+    return {name: 0 if params.strip() in ("", "void") else params.count(",") + 1
+            for name, params in re.findall(r"\b(rp_[a-z0-9_]+)\s*\(([^)]*)\)", txt)}
+
+
+def test_binding_declares_every_function_with_the_header_parameter_count():
+    counts = declared_parameter_counts()
+    assert sorted(counts) == declared_symbols()
+    assert sorted(api.SIGNATURES) == sorted(counts), "the binding's table and include/racon_b200.h name other functions"
+    wrong = {s: (n, len(api.SIGNATURES[s][1])) for s, n in counts.items() if len(api.SIGNATURES[s][1]) != n}
+    assert not wrong, "parameters in the header vs argtypes in racon_b200/api.py: %s" % wrong
+
+
 def test_library_builds_and_exports_every_declared_symbol():
     path = build.build_cuda()
     lib = C.CDLL(path)

@@ -51,8 +51,6 @@ def test_fasta_record_format_reproduces_racon_stdout():
     import hashlib
     from racon_b200 import api
     lib = api.load()
-    lib.rp_mirror_format_fasta.restype = C.c_uint64
-    lib.rp_mirror_format_fasta.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64]
     ref = np.load(os.path.join(GOLD, "lambda_windows.npz"))
     full = ref["polished_name"].tobytes()
     cut = full.index(b" LN:i:")
