@@ -41,7 +41,8 @@ enum {
     RP_WIN_NODE_LIMIT = 1,
     RP_WIN_EDGE_LIMIT = 2,
     RP_WIN_ALIGNED_LIMIT = 3,
-    RP_WIN_NEEDS_INT32 = 4,      /* the score matrix really leaves int16 (|gap| > 64, or |gap| * (graph depth + length) > ~31k) */
+    RP_WIN_NEEDS_INT32 = 4,      /* the score matrix may leave int16 (|gap| > 64, |gap| * (graph depth + length) > ~31k, or
+                                    max(match, mismatch) * length > ~31k) */
     RP_WIN_SEQ_TOO_LONG = 5,
     RP_WIN_STACK_LIMIT = 6,
     RP_WIN_ALPHABET_LIMIT = 7,

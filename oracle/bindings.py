@@ -56,6 +56,10 @@ def oracle_lib():
             lib.oracle_myers_cigar.restype = C.c_int64
             lib.oracle_myers_cigar.argtypes = [C.c_char_p, C.c_uint32, C.c_char_p, C.c_uint32, C.c_void_p,
                                                C.c_uint64, C.c_void_p]
+        lib.oracle_poa_trace_begin.restype = None
+        lib.oracle_poa_trace_begin.argtypes = []
+        lib.oracle_poa_trace_end.restype = C.c_uint64
+        lib.oracle_poa_trace_end.argtypes = [C.c_void_p, C.c_uint64]
         if hasattr(lib, "oracle_breaking_points"):
             lib.oracle_breaking_points.restype = C.c_int64
             lib.oracle_breaking_points.argtypes = [C.c_char_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32,
@@ -107,6 +111,24 @@ def oracle_consensus(ws, m=3, x=-5, g=-4, window_length=500, trim=True, threads=
     if want_coverage:
         return cons, pol, secs, [cov[w, :len(cons[w])].copy() for w in range(n)]
     return cons, pol, secs
+
+
+def oracle_matrix_ranges(ws, m=3, x=-5, g=-4, window_length=500, trim=True):
+    """Per window, an (alignments, 5) int64 array: read length, graph rows, lowest column-0 value, lowest and highest
+    cell of each of the window's int32 score matrices, in the order the oracle aligned its layers."""
+    lib = oracle_lib()
+    out = []
+    for w in range(ws.n_windows):
+        sub = ws.subset([w])
+        lib.oracle_poa_trace_begin()
+        try:
+            _run(lib.oracle_poa_consensus, sub, m, x, g, window_length, trim, 1, extra=(None,))
+        finally:
+            cap = int(ws.win_first[w + 1] - ws.win_first[w])
+            rec = np.zeros((cap, 5), np.int64)
+            n = lib.oracle_poa_trace_end(rec.ctypes.data, cap)
+        out.append(rec[:min(n, cap)])
+    return out
 
 
 def ref_edlib_cigar(q, t):

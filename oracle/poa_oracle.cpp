@@ -40,6 +40,11 @@ struct Stats {
 };
 Stats g_stats;
 
+/* oracle_poa_trace_begin/_end: while on, every alignment appends (read length, graph rows, lowest column-0 value, lowest
+ * and highest cell) of its finished int32 matrix.  Single-threaded runs only (n_threads == 1). */
+bool g_trace_on = false;
+std::vector<int64_t> g_trace;
+
 struct Edge {
     uint32_t tail, head;
     int64_t weight;
@@ -385,6 +390,15 @@ struct Engine {
         g_stats.pred_rows += prow;
         if (n_sinks > 1) g_stats.multi_sink++;
         if (n_tied > 1) g_stats.sink_ties++;
+        if (g_trace_on) {
+            int64_t col0 = 0, lo = H[0], hi = H[0];
+            for (uint64_t c = 0; c < W * (n + 1); ++c) {
+                lo = std::min<int64_t>(lo, H[c]);
+                hi = std::max<int64_t>(hi, H[c]);
+                if (c % W == 0) col0 = std::min<int64_t>(col0, H[c]);
+            }
+            g_trace.insert(g_trace.end(), {static_cast<int64_t>(len), static_cast<int64_t>(n), col0, lo, hi});
+        }
         if (max_i == 0 && max_j == 0) return alignment;
 
         uint32_t i = max_i, j = max_j, prev_i = 0, prev_j = 0;
@@ -592,6 +606,19 @@ void oracle_poa_stats(uint64_t* out) {
     out[9] = g_stats.max_aligned.exchange(0);
     out[10] = g_stats.far_pred_rows.exchange(0);
     out[11] = g_stats.pred_rows.exchange(0);
+}
+
+void oracle_poa_trace_begin(void) {
+    g_trace.clear();
+    g_trace_on = true;
+}
+
+/* Stops the trace; copies up to `cap` records of 5 int64 (see g_trace) to `out` and returns how many were taken. */
+uint64_t oracle_poa_trace_end(int64_t* out, uint64_t cap) {
+    g_trace_on = false;
+    const uint64_t n = g_trace.size() / 5;
+    std::memcpy(out, g_trace.data(), std::min(n, cap) * 5 * sizeof(int64_t));
+    return n;
 }
 
 }  // extern "C"

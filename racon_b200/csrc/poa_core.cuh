@@ -743,7 +743,7 @@ struct PoaWarp {
     /* True iff no cell of the finished matrix can have left the range int16 arithmetic is exact in.  Every cell
      * satisfies H[i][j] >= H[i][0] + j*g (the horizontal move is always a candidate), column 0 falls by exactly |g|
      * per level along a shortest path (so it cannot jump over the limit unnoticed), and the largest value is bounded
-     * by match * min(rows, columns), checked by the caller.  Limit: spoa's own margin, -32768 + 1024. */
+     * by max(match, mismatch) * min(rows, columns), checked by the caller.  Limit: spoa's own margin, -32768 + 1024. */
     RP_DEV bool matrix_in_range(uint32_t nrows, uint32_t len, uint32_t lpa) {
         int32_t mn = 0;
         const uint32_t e0 = perm(0);
@@ -2244,18 +2244,18 @@ RP_DEV void poa_window(const PoaParams& P, uint32_t w, uint8_t* slot, uint8_t* s
         /* spoa picks its int32 engine from a worst-case bound over ALL nodes of the graph (fits_int16).  That bound
          * is far from what a real matrix holds (column 0 only falls by |g| per level of graph DEPTH), and exact
          * arithmetic gives the same answer in either width, so a window that fails the bound is still computed in
-         * int16 and the finished matrix is checked for having stayed in range (matrix_in_range). */
-        bool verify_range = false;
+         * int16 and the finished matrix is checked for having stayed in range (matrix_in_range).  The bound says
+         * nothing about the top of the range: a long copy of the read scores up to max(match, mismatch) per column even
+         * where the bound holds (a deep graph), and spoa's int16 engine wraps there, so such a window is refused. */
         const int64_t worst = worst_case_score(P.match, P.gap, len, nrows);
         const bool fits = P.gap >= -kMaxGapInt16 && worst >= static_cast<int64_t>(-32768 + 1024);
-        if (!fits) {
-            const int64_t short_side = static_cast<int64_t>(len) + 8 < nrows ? static_cast<int64_t>(len) + 8 : nrows;
-            if (P.gap < -kMaxGapInt16 || static_cast<int64_t>(P.match) * short_side > 32767 - 1024) {
-                W.fail(kWinNeedsInt32);
-                break;
-            }
-            verify_range = true;
+        const int64_t short_side = static_cast<int64_t>(len) + 8 < nrows ? static_cast<int64_t>(len) + 8 : nrows;
+        const int64_t top_step = P.match > P.mismatch ? (P.match > 0 ? P.match : 0) : (P.mismatch > 0 ? P.mismatch : 0);
+        if (P.gap < -kMaxGapInt16 || top_step * short_side > 32767 - 1024) {
+            W.fail(kWinNeedsInt32);
+            break;
         }
+        const bool verify_range = !fits;
         const uint32_t lpa = (len + 1 + kCC - 1) / kCC * kCC;
         /* shared memory (chunk-local): profile chunk | ring of the last R DP rows; the traceback re-uses it */
         const uint32_t prof_bytes = W.ncodes * kCC * 2;

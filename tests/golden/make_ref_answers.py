@@ -20,6 +20,10 @@ def main():
         for scores in to.SCORES:
             poa["%s/%d,%d,%d" % ((name,) + scores)] = util.consensus_answer(*to.equals_reference_case(name, scores)(
                 ob.ref_consensus))
+    for name in sorted(to.EXTREME_SCORES):
+        for scores in to.EXTREME_SCORES[name]:
+            poa["%s/%d,%d,%d" % ((name,) + scores)] = util.consensus_answer(*to.equals_reference_case(name, scores)(
+                ob.ref_consensus))
     poa["partial/no_trim"] = util.consensus_answer(*to.no_trim_case()(ob.ref_consensus))
     edlib = {}
     for n, err, count in tm.TRACEBACK:

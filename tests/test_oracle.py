@@ -82,6 +82,13 @@ def equals_reference_case(name, scores):
     return lambda consensus: consensus(ws, m, x, g, window_length=wl, threads=8)[:2]
 
 
+# racon takes any int8 -m/-x/-g: gap 0, match <= 0, mismatch >= match, mismatch -128, match 127 (127 only on short windows:
+# on long ones spoa's own int16 engine wraps at the top of its range)
+EXTREME_SCORES = {"shallow": [(3, -5, 0), (0, -1, -1), (2, 3, -1), (-1, -2, -3), (127, -128, -1), (1, -128, -64),
+                              (10, -1, -20)],
+                  "partial_qual": [(3, -5, 0), (2, 3, -1), (-1, -2, -3)]}
+
+
 def no_trim_case():
     ws = _mk("partial", seed=7)
     return lambda consensus: consensus(ws, trim=False, threads=4)[:2]
@@ -90,6 +97,11 @@ def no_trim_case():
 @pytest.mark.parametrize("name", sorted(CASES))
 @pytest.mark.parametrize("scores", SCORES)
 def test_oracle_equals_reference(name, scores):
+    _check("%s/%d,%d,%d" % ((name,) + scores), equals_reference_case(name, scores))
+
+
+@pytest.mark.parametrize("name,scores", [(n, s) for n in sorted(EXTREME_SCORES) for s in EXTREME_SCORES[n]])
+def test_oracle_equals_reference_extreme_scores(name, scores):
     _check("%s/%d,%d,%d" % ((name,) + scores), equals_reference_case(name, scores))
 
 
