@@ -157,7 +157,9 @@ rp_status rp_poa_enable_counters(rp_poa* p, int on);
  * in columns, [4] (only with the environment variable RP_BAND_AUDIT=1, a test mode that recomputes every accepted
  * band result with the full matrix) accepted band alignments that differ from the full-matrix alignment, [5] 1 when the
  * band layout is in use: a banded object uses it for windows of 768 bases or more (where it is the faster kernel) or when
- * RP_POA_BAND_K / RP_POA_GROUP ask for it; otherwise -b runs the full matrix, which returns the same results faster.
+ * the environment variables RP_POA_BAND_K (band columns per lane) / RP_POA_GROUP (lanes per window) ask for it; each
+ * layout has a kernel and a launch shape of its own.  Otherwise -b runs the full matrix, which returns the same results
+ * faster.
  * Banded and unbanded objects return identical results (tests/test_gpu_poa.py). */
 rp_status rp_poa_band_info(rp_poa* p, uint64_t info[8]);
 

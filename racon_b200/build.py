@@ -77,8 +77,6 @@ def build_cuda(force=False, verbose=False):
             "-o", out] + cu
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
-        extra = os.environ.get("RP_NVCC_DEFINES", "").split()   # A/B switches of the kernels (csrc/poa_core.cuh)
-        cmd[1:1] = extra
         log = _run(cmd)
         if verbose:
             print(log)

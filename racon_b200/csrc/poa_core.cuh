@@ -30,22 +30,6 @@
  */
 #pragma once
 #include "rp_warp.cuh"
-#if defined(RP_HOST_SIM)
-#include <vector>
-#endif
-
-/* A/B switches for measuring the round-2 (DESIGN.md 11a) changes one by one on the device; all on by default, set with
- * RP_NVCC_DEFINES="-DRP_POA_SERIAL_WALK_MAX=0 -DRP_POA_PREV_ROW=0 -DRP_POA_ASYNC_REFILL=0" python -c 'from racon_b200 import
- * build; build.build_cuda(force=True)' (results are identical either way). */
-#ifndef RP_POA_SERIAL_WALK_MAX
-#define RP_POA_SERIAL_WALK_MAX 7   /* rows with up to this many predecessors: candidates walked serially (0: only root rows) */
-#endif
-#ifndef RP_POA_PREV_ROW
-#define RP_POA_PREV_ROW 1          /* a predecessor that is the row just computed comes from registers */
-#endif
-#ifndef RP_POA_ASYNC_REFILL
-#define RP_POA_ASYNC_REFILL 1      /* traceback tile refill by cp.async */
-#endif
 
 namespace rp {
 
@@ -221,19 +205,6 @@ struct alignas(16) U4 {
 struct alignas(8) U2 {
     uint32_t x, y;
 };
-#if defined(RP_HOST_SIM)
-static unsigned long g_sim_scan_rows = 0, g_sim_scan_full = 0;   // simulation only: how often the full carry scan runs
-#define RP_SIM_COUNT(x) do { if (lane == 0) ++(x); } while (0)
-#else
-#define RP_SIM_COUNT(x) do { } while (0)
-#endif
-#if defined(RP_HOST_SIM)
-/* simulation only (debug_flags bit 3): copies for the band audit's diagnosis of a differing alignment */
-struct AuditStep { uint32_t i, j, move, p; int32_t h; };
-static std::vector<AuditStep> g_audit_path[2];
-static std::vector<int16_t> g_audit_h;
-static std::vector<uint8_t> g_audit_bs;
-#endif
 
 /* A lane's 16 columns = two 16-byte granules 2*lane, 2*lane+1 of the row (chunk or band) it belongs to */
 RP_DEV Row8 load_row_smem(const int16_t* row, int lane) {
@@ -862,7 +833,7 @@ struct PoaWarp {
                  * more predecessors enter the nested part */
                 {
                     const uint32_t p0 = np ? (lo >> 16) : 0u;
-                    if (RP_POA_PREV_ROW && p0 + 1 == i && p0 != 0) {  // group-uniform
+                    if (p0 + 1 == i && p0 != 0) {  // group-uniform
                         /* the first predecessor is the row just computed (4 of 10 rows): it still is in registers — no
                          * trip through the shared-memory ring, whose store -> load latency would start this row */
                         pm = prev;
@@ -928,9 +899,7 @@ struct PoaWarp {
                     }
                     carry = shfl_up(t, 1);
                     carry = lanem == 0 ? chunk_carry : carry;
-                    RP_SIM_COUNT(g_sim_scan_full);
                 }
-                RP_SIM_COUNT(g_sim_scan_rows);
                 carry = carry < negsafe ? negsafe : carry;
                 const uint32_t c2 = pack16(carry, carry);
 #pragma unroll
@@ -1452,9 +1421,6 @@ struct PoaWarp {
         const U4 f4 = U4{pack16(kBandFloor, kBandFloor), pack16(kBandFloor, kBandFloor), pack16(kBandFloor, kBandFloor),
                          pack16(kBandFloor, kBandFloor)};
         uint32_t i = best_row, j = len;
-#if defined(RP_HOST_SIM)
-        if (lane == 0) g_audit_path[BAND ? 1 : 0].clear();
-#endif
         uint32_t t_top = 0, t_rows = 0, t_col0 = 0;  // tile covers ranks (t_top - t_rows, t_top], cols [t_col0, t_col0+32)
         bool have_tile = false, bad = false;
         uint32_t quality = 0;
@@ -1500,38 +1466,34 @@ struct PoaWarp {
                 }
                 /* four lanes per tile row, one 16-byte granule each: consecutive lanes write consecutive 16-byte
                  * granules of the tile (no shared-memory bank conflict) and read one 64-byte piece of an H row.
-                 * Full matrix: asynchronous copies (cp.async), all of a lane's granules — up to 12 — in flight at once;
-                 * the loop used to wait one HBM latency per granule (a load into registers, then the store). */
+                 * Full matrix: asynchronous copies (cp.async), all of a lane's granules — up to 12 — in flight at once.
+                 * Band: through registers, which substitute the out-of-band granules. */
                 for (uint32_t e = lane; e < 4 * t_rows; e += G) {
                     const uint32_t q = e >> 2, gq = e & 3u;
                     const uint32_t rk = t_top - q;
-                    if (!BAND && RP_POA_ASYNC_REFILL) {
+                    if (!BAND) {
                         copy16_async(reinterpret_cast<U4*>(tile) + e,
                                      reinterpret_cast<const U4*>(H + static_cast<uint64_t>(rk) * lpa + t_col0) + gq);
                         continue;
                     }
                     U4 v;
-                    if (!BAND) {
-                        v = reinterpret_cast<const U4*>(H + static_cast<uint64_t>(rk) * lpa + t_col0)[gq];
-                    } else {
-                        const uint32_t sr = bs[rk];
-                        const uint32_t blk = cba + (gq >> 1);
-                        if (rk == 0) {  // virtual root row: H[0][c] = c * g, in the row's register order
-                            int16_t t8[8];
+                    const uint32_t sr = bs[rk];
+                    const uint32_t blk = cba + (gq >> 1);
+                    if (rk == 0) {  // virtual root row: H[0][c] = c * g, in the row's register order
+                        int16_t t8[8];
 #pragma unroll
-                            for (uint32_t k = 0; k < 8; ++k) {
-                                const uint32_t el = (gq & 1u) * 8 + k;                  // element inside the block
-                                const uint32_t col = blk * 16 + unperm_band(el);
-                                t8[k] = static_cast<int16_t>(static_cast<int32_t>(col) * g);
-                            }
-                            v = U4{pack16(t8[0], t8[1]), pack16(t8[2], t8[3]), pack16(t8[4], t8[5]), pack16(t8[6], t8[7])};
-                        } else {
-                            /* the granule's address does not depend on the row's band start: both loads go out together */
-                            v = reinterpret_cast<const U4*>(H + static_cast<uint64_t>(rk) * kBW + ((blk & (NB - 1)) << 4))[gq & 1u];
-                            if (blk - sr >= NB) v = f4;
+                        for (uint32_t k = 0; k < 8; ++k) {
+                            const uint32_t el = (gq & 1u) * 8 + k;                  // element inside the block
+                            const uint32_t col = blk * 16 + unperm_band(el);
+                            t8[k] = static_cast<int16_t>(static_cast<int32_t>(col) * g);
                         }
-                        if (gq == 0) tbs[q] = static_cast<uint8_t>(sr);
+                        v = U4{pack16(t8[0], t8[1]), pack16(t8[2], t8[3]), pack16(t8[4], t8[5]), pack16(t8[6], t8[7])};
+                    } else {
+                        /* the granule's address does not depend on the row's band start: both loads go out together */
+                        v = reinterpret_cast<const U4*>(H + static_cast<uint64_t>(rk) * kBW + ((blk & (NB - 1)) << 4))[gq & 1u];
+                        if (blk - sr >= NB) v = f4;
                     }
+                    if (gq == 0) tbs[q] = static_cast<uint8_t>(sr);
                     reinterpret_cast<U4*>(tile)[e] = v;
                 }
                 if (G == 32) {
@@ -1543,7 +1505,7 @@ struct PoaWarp {
                 } else {
                     for (uint32_t q = lane; q < t_rows; q += G) trec[q] = rec[t_top - q];
                 }
-                if (!BAND && RP_POA_ASYNC_REFILL) copy_async_wait();
+                if (!BAND) copy_async_wait();
                 have_tile = true;
                 syncwarp();
             }
@@ -1567,8 +1529,7 @@ struct PoaWarp {
             if (j > 0) mc = cidx == tile_b[tseq_at + j - 1] ? m : x;
             uint32_t found_p = 0;
             int move = 0;  // 1 diag, 2 vert, 3 horiz
-            static_assert(RP_POA_SERIAL_WALK_MAX <= 7, "only the predecessors held in the record are walked serially");
-            if (np <= RP_POA_SERIAL_WALK_MAX) {  // group-uniform: every predecessor is in the row's record
+            if (np <= 7) {  // group-uniform: every predecessor is in the row's record
                 /* 7 of 10 steps of the walk are on rows with several predecessors (the consensus path runs through the
                  * nodes many reads agree on), and on nearly all of them the FIRST in-edge — the oldest, heaviest one — is the
                  * diagonal match.  So the lanes do not spread the candidates over themselves and vote: every lane walks
@@ -1689,9 +1650,6 @@ struct PoaWarp {
                     break;
                 }
             }
-#if defined(RP_HOST_SIM)
-            if ((P->debug_flags & 8u) && lane == 0) g_audit_path[BAND ? 1 : 0].push_back({i, j, static_cast<uint32_t>(move), found_p, hij});
-#endif
             if (move == 1) {
                 put_aln(j - 1, i);   // rank for now, node below
                 i = found_p;
@@ -2294,13 +2252,8 @@ RP_DEV void poa_window(const PoaParams& P, uint32_t w, uint8_t* slot, uint8_t* s
             }
             if (done) done = W.template traceback<true>(best_row, len, lpa, seq, sub, static_cast<int32_t>(worst));
             if (P.band_stats && lane == 0) {
-#if !defined(RP_HOST_SIM)
-                atomicAdd(P.band_stats, 1ull);
-                if (!done) atomicAdd(P.band_stats + 1, 1ull);
-#else
-                P.band_stats[0] += 1;
-                if (!done) P.band_stats[1] += 1;
-#endif
+                count_add(P.band_stats, 1);
+                if (!done) count_add(P.band_stats + 1, 1);
             }
             if (W.status != kWinOk) break;
         }
@@ -2310,13 +2263,6 @@ RP_DEV void poa_window(const PoaParams& P, uint32_t w, uint8_t* slot, uint8_t* s
             for (uint32_t c = lane; c < len; c += G) W.cur[c] = W.aln[c];
             W.syncwarp();
             done = false;
-#if defined(RP_HOST_SIM)
-            if ((P.debug_flags & 8u) && lane == 0) {
-                g_audit_h.assign(W.H, W.H + static_cast<size_t>(nrows + 1) * kBW);
-                g_audit_bs.assign(W.bs, W.bs + nrows + 1);
-            }
-            W.syncwarp();
-#endif
         }
         if (!done) {
             if (static_cast<uint64_t>(nrows + 1) * lpa > P.lim.hcap) {
@@ -2336,64 +2282,7 @@ RP_DEV void poa_window(const PoaParams& P, uint32_t w, uint8_t* slot, uint8_t* s
             if (audit) {
                 bool diff = false;
                 for (uint32_t c = lane; c < len; c += G) diff |= W.cur[c] != W.aln[c];
-                if (W.ballot(diff) && lane == 0 && P.band_stats) {
-#if !defined(RP_HOST_SIM)
-                    atomicAdd(P.band_stats + 2, 1ull);
-#else
-                    P.band_stats[2] += 1;
-                    if (P.debug_flags & 8u) {
-                        auto hbv = [&](uint32_t r, uint32_t c) -> int32_t {
-                            if (r == 0) return static_cast<int32_t>(c) * P.gap;
-                            const uint32_t cbk = c >> 4;
-                            if (cbk - g_audit_bs[r] >= NB) return -99999;
-                            return g_audit_h[static_cast<size_t>(r) * kBW + ((cbk & (NB - 1)) << 4) + (PW::perm_band(c) & 15u)];
-                        };
-                        const auto& pb = g_audit_path[1];
-                        const auto& pf = g_audit_path[0];
-                        fprintf(stderr, "[band audit] window %u layer %u: len %u rows %u sub %d, full best %d; band path %zu steps, full path %zu steps\n",
-                                w, s - s0, len, nrows, sub ? 1 : 0, best, pb.size(), pf.size());
-                        size_t k = 0;
-                        while (k < pb.size() && k < pf.size() && pb[k].i == pf[k].i && pb[k].j == pf[k].j && pb[k].move == pf[k].move && pb[k].p == pf[k].p) ++k;
-                        if (k < pb.size() && k < pf.size()) {
-                            fprintf(stderr, "    DIVERGE at step %zu: cell (rank %u, col %u) h band %d full %d; band move %u -> %u, full move %u -> %u; band cols [%u,%u)\n",
-                                    k, pb[k].i, pb[k].j, pb[k].h, pf[k].h, pb[k].move, pb[k].p, pf[k].move, pf[k].p,
-                                    16u * g_audit_bs[pb[k].i], 16u * (g_audit_bs[pb[k].i] + NB));
-                            const uint32_t i0 = pf[k].i, j0 = pf[k].j;
-                            const Rec rc = W.rec[i0];
-                            const uint32_t np = (static_cast<uint32_t>(rc.a) >> 8) & 0x7f;
-                            for (uint32_t q = 0; q < np; ++q) {
-                                const uint32_t pp = q < 7 ? rec_pred(rc, q) : W.pred_ovf[i0 * W.ki + q];
-                                fprintf(stderr, "      pred %u rank %u band cols [%u,%u): band (j-1) %d (j) %d | full (j-1) %d (j) %d\n", q, pp,
-                                        16u * g_audit_bs[pp], 16u * (g_audit_bs[pp] + NB), hbv(pp, j0 ? j0 - 1 : 0), hbv(pp, j0),
-                                        static_cast<int>(W.H[static_cast<uint64_t>(pp) * lpa + perm(j0 ? j0 - 1 : 0)]),
-                                        static_cast<int>(W.H[static_cast<uint64_t>(pp) * lpa + perm(j0)]));
-                            }
-                        }
-                        /* where along the FULL path is the band value lower (or the cell outside the band)? */
-                        int shown = 0, n_out = 0, far = 0;
-                        uint32_t first_out_j = 0, last_out_j = 0;
-                        for (const auto& st : pf) {
-                            const int32_t lo_c = 16 * g_audit_bs[st.i], hi_c = 16 * (g_audit_bs[st.i] + NB);
-                            const int32_t jj = st.j;
-                            if (jj < lo_c || jj >= hi_c) {
-                                ++n_out;
-                                const int d = jj < lo_c ? lo_c - jj : jj - hi_c + 1;
-                                if (d > far) far = d;
-                                if (!last_out_j) last_out_j = st.j;
-                                first_out_j = st.j;
-                            }
-                        }
-                        fprintf(stderr, "    full path: %d cells outside the band (columns %u..%u), farthest %d columns beyond the edge\n",
-                                n_out, first_out_j, last_out_j, far);
-                        for (const auto& st : pf) {
-                            const int32_t hb = hbv(st.i, st.j);
-                            if (hb != st.h && shown++ < 4)
-                                fprintf(stderr, "    full-path cell (rank %u, col %u): full %d band %d, band cols [%u,%u)\n", st.i, st.j, st.h, hb,
-                                        16u * g_audit_bs[st.i], 16u * (g_audit_bs[st.i] + NB));
-                        }
-                    }
-#endif
-                }
+                if (W.ballot(diff) && lane == 0 && P.band_stats) count_add(P.band_stats + 2, 1);
             }
         }
         W.add_alignment(seq, wts, len, b0);
@@ -2401,17 +2290,10 @@ RP_DEV void poa_window(const PoaParams& P, uint32_t w, uint8_t* slot, uint8_t* s
         if (P.stats) pred_rows = W.shfl(pred_rows, G - 1);
         if (P.stats && lane == 0) {
             const unsigned long long cols = (band && done) ? kBW : len + 1;   // columns the accepted DP computed per row
-#if !defined(RP_HOST_SIM)
-            atomicAdd(reinterpret_cast<unsigned long long*>(P.stats + 3), static_cast<unsigned long long>(pred_rows) * cols);
-            atomicAdd(reinterpret_cast<unsigned long long*>(P.stats), 1ull);
-            atomicAdd(reinterpret_cast<unsigned long long*>(P.stats + 1), static_cast<unsigned long long>(nrows + 1) * cols);
-            if (n_best > 1) atomicAdd(reinterpret_cast<unsigned long long*>(P.stats + 2), 1ull);
-#else
-            P.stats[0] += 1;
-            P.stats[3] += static_cast<uint64_t>(pred_rows) * cols;
-            P.stats[1] += static_cast<uint64_t>(nrows + 1) * cols;
-            if (n_best > 1) P.stats[2] += 1;
-#endif
+            count_add(P.stats + 3, pred_rows * cols);
+            count_add(P.stats, 1);
+            count_add(P.stats + 1, (nrows + 1) * cols);
+            if (n_best > 1) count_add(P.stats + 2, 1);
         }
     }
     uint32_t clen = 0;

@@ -153,10 +153,16 @@ rp_status set_stream(StreamOwner* o, void* cuda_stream) {
 constexpr int kWarpsPerBlock = 4;
 constexpr uint32_t kBandPaysFromWindowLength = 768;   // rows of two or more 512-column chunks
 
+/* Blocks per SM of the POA kernel, which sets its register cap, by columns per lane of a row.  Measured on the H100
+ * (DESIGN.md §11b): 16 columns (the full matrix, and the 8- and 16-lane bands) run best at 3 — at 4 the 128-register cap
+ * makes ptxas spill inside the DP row loop on sm_90a; the narrow 32 x 8 and 32 x 4 bands need fewer registers per row
+ * and run best at 5. */
+constexpr int poa_blocks_per_sm(int kb) { return kb == 16 ? 3 : 5; }
+
 /* Persistent kernel: every GROUP of G lanes (G = 8, 16, 32; rp_warp.cuh) is an independent worker that pulls
  * windows from an atomic queue — 32/G windows in flight per warp, advancing together wherever their control
- * flow agrees.  Compiled for several group widths and occupancy points (blocks per SM -> register cap);
- * RP_POA_GROUP / RP_BLOCKS_PER_SM select one (defaults in rp_poa_create). */
+ * flow agrees.  Compiled for each layout (lanes per window x columns per lane of a row); RP_POA_GROUP /
+ * RP_POA_BAND_K select one (defaults in configure). */
 #if defined(RP_HOST_SIM)
 /* TEST-ONLY stand-ins of the two kernels (cuda_sim_runtime.h): the same per-window / per-overlap device functions, run as
  * cooperative fibres, the queue walked by one worker after the other. */
@@ -173,7 +179,7 @@ struct SimPoaJob {
         rp::poa_window<G, KB>(*j->P, j->w, j->slot, j->smem);
     }
 };
-template <int G, int KB, int kBlocksPerSm>
+template <int G, int KB>
 void rp_poa_kernel(rp::PoaParams P, SimLaunch L) {
     const uint32_t workers = L.blocks * (L.threads / G);
     std::vector<uint8_t> smem(P.smem_per_group + 64);
@@ -225,7 +231,9 @@ cudaError_t launch(void (*kernel)(Params, SimLaunch), uint32_t blocks, uint32_t 
     return cudaSuccess;
 }
 #else
-template <int G, int KB, int kBlocksPerSm>
+/* kBlocksPerSm is fixed by the layout; it stays a template argument so that the kernel keeps its symbol name
+ * (rp_poa_kernel<G, KB, blocks per SM>), by which tools/sass_by_line.py, the SASS tests and profiles find it */
+template <int G, int KB, int kBlocksPerSm = poa_blocks_per_sm(KB)>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSm) rp_poa_kernel(rp::PoaParams P) {
     extern __shared__ __align__(16) uint8_t smem_all[];
     const uint32_t grp = threadIdx.x / G;
@@ -248,39 +256,13 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSm) rp_poa_kern
 
 typedef void (*PoaKernel)(rp::PoaParams);
 #endif
-/* lanes per window x columns per lane of a banded row x blocks per SM (register cap) */
-template <int G, int KB>
-PoaKernel pick_kernel_g(int blocks_per_sm) {
-    switch (blocks_per_sm) {
-        case 2: return rp_poa_kernel<G, KB, 2>;
-        case 4: return rp_poa_kernel<G, KB, 4>;
-        case 6: return rp_poa_kernel<G, KB, 6>;
-        default: return rp_poa_kernel<G, KB, 3>;
-    }
-}
-template <int KB>
-PoaKernel pick_kernel_narrow(int blocks_per_sm) {   // 32 lanes, narrow banded rows: few registers per row
-    switch (blocks_per_sm) {
-        case 4: return rp_poa_kernel<32, KB, 4>;
-        case 6: return rp_poa_kernel<32, KB, 6>;
-        case 8: return rp_poa_kernel<32, KB, 8>;
-        default: return rp_poa_kernel<32, KB, 5>;
-    }
-}
-PoaKernel pick_kernel(int group, int band_k, int blocks_per_sm) {
-#if defined(RP_ONLY_DEFAULT_KERNEL)
-    /* development builds for SASS inspection (tools/sass_by_line.py --quick): one instantiation, seconds to compile */
-    (void)group; (void)band_k; (void)blocks_per_sm;
-    return rp_poa_kernel<32, 16, 3>;
-#else
-    if (group == 32 && band_k == 4) return pick_kernel_narrow<4>(blocks_per_sm);
-    if (group == 32 && band_k == 8) return pick_kernel_narrow<8>(blocks_per_sm);
-    switch (group) {
-        case 8: return pick_kernel_g<8, 16>(blocks_per_sm);
-        case 16: return pick_kernel_g<16, 16>(blocks_per_sm);
-        default: return pick_kernel_g<32, 16>(blocks_per_sm);
-    }
-#endif
+/* lanes per window x columns per lane of a row (band_k is 16 unless group is 32) */
+PoaKernel pick_kernel(int group, int band_k) {
+    if (group == 8) return rp_poa_kernel<8, 16>;
+    if (group == 16) return rp_poa_kernel<16, 16>;
+    if (band_k == 4) return rp_poa_kernel<32, 4>;
+    if (band_k == 8) return rp_poa_kernel<32, 8>;
+    return rp_poa_kernel<32, 16>;
 }
 
 #if !defined(RP_HOST_SIM)
@@ -396,7 +378,6 @@ struct rp_poa : StreamOwner {
     int grid = 0;
     uint32_t smem_block = 0;
     PoaKernel kernel = nullptr;
-    int blocks_per_sm = 4;
     int group = 32;                // lanes per window
     int band_k = 16;               // columns per lane of a banded row
     uint32_t groups_per_block = 4;
@@ -515,12 +496,11 @@ static rp_status configure(rp_poa* p, uint32_t wl) {
     /* tests only: recompute every accepted band result with the full matrix and count the differences */
     if (const char* e_a = getenv("RP_BAND_AUDIT")) p->P.debug_flags = atoi(e_a) ? 2u : 0u;
 
-    /* launch shape: persistent blocks of 4 warps = 128/G lane groups, kBlocksPerSm blocks per SM.  Defaults measured on
-     * the H100 (tools/tune_poa.py, 10 000 windows of bench config 2): full matrix: 32 lanes per window, 16 columns per
-     * lane, 3 blocks/SM — at 4 blocks/SM the 128-register cap makes ptxas spill on sm_90a and the kernel is ~3 % slower;
-     * banded (-b): 32 lanes x 8 columns = a 256-column band (the width of cudapoa's static band) — four packed registers
-     * per row instead of eight — at 5 blocks/SM.  RP_POA_BAND_K=4 selects a 128-column band (faster on clean data,
-     * refuses more often). */
+    /* launch shape: persistent blocks of 4 warps = 128/G lane groups, poa_blocks_per_sm blocks per SM.  Defaults measured
+     * on the H100 (tools/tune_poa.py, 10 000 windows of bench config 2): full matrix: 32 lanes per window, 16 columns per
+     * lane; banded (-b): 32 lanes x 8 columns = a 256-column band (the width of cudapoa's static band) — four packed
+     * registers per row instead of eight.  RP_POA_BAND_K=4 selects a 128-column band (faster on clean data, refuses more
+     * often). */
     int group = 32;
     if (const char* e_g = getenv("RP_POA_GROUP")) group = atoi(e_g);
     if (group != 8 && group != 16 && group != 32) group = 32;
@@ -534,20 +514,12 @@ static rp_status configure(rp_poa* p, uint32_t wl) {
     const bool band_forced = getenv("RP_POA_BAND_K") != nullptr || getenv("RP_POA_GROUP") != nullptr;
     p->P.banded = (banded && (band_forced || wl >= kBandPaysFromWindowLength)) ? 1 : 0;
     if (!p->P.banded) band_k = 16;
-    int bps = band_k == 16 ? 3 : 5;
-    if (const char* e_bps = getenv("RP_BLOCKS_PER_SM")) bps = atoi(e_bps);
-    if (band_k == 16) {
-        if (bps != 2 && bps != 4 && bps != 6) bps = 3;
-    } else if (bps != 4 && bps != 6 && bps != 8) {
-        bps = 5;
-    }
     p->group = group;
     p->band_k = band_k;
     p->groups_per_block = kWarpsPerBlock * 32 / group;
-    p->blocks_per_sm = bps;
-    p->kernel = pick_kernel(group, band_k, bps);
+    p->kernel = pick_kernel(group, band_k);
     uint32_t smem_per_sm = static_cast<uint32_t>(prop.sharedMemPerMultiprocessor);
-    uint32_t per_block = smem_per_sm / bps - 1024;                              // 1 KB reserved per block
+    uint32_t per_block = smem_per_sm / poa_blocks_per_sm(band_k) - 1024;       // 1 KB reserved per block
     if (per_block > prop.sharedMemPerBlockOptin) per_block = static_cast<uint32_t>(prop.sharedMemPerBlockOptin);
     uint32_t per_group = (per_block / p->groups_per_block) & ~255u;
     p->P.smem_per_group = per_group;
@@ -578,7 +550,6 @@ static rp_status configure(rp_poa* p, uint32_t wl) {
         hcap = per > fixed_bytes + 4096 ? (per - fixed_bytes - 4096) / 2 : 0;
         hcap = std::max(hcap_min, std::min(hcap, hcap_full));
     }
-    if (const char* e_h = getenv("RP_POA_HCAP")) hcap = std::max<uint64_t>(1024, strtoull(e_h, nullptr, 10));
     lim.hcap = static_cast<uint32_t>(std::min<uint64_t>(hcap, 0xfffffff0ull));
     p->P.lim = lim;
     p->P.lay = rp::make_layout(lim);

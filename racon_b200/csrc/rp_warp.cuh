@@ -168,6 +168,9 @@ inline uint32_t atomic_add_u16(uint16_t* p, uint32_t v) {
     *p = static_cast<uint16_t>(o + v);
     return o;
 }
+/* adds v to a 64-bit statistics counter (atomic on the device; here the workers run one after the other) */
+template <typename T>
+inline void count_add(T* p, unsigned long long v) { *p += v; }
 inline int popc(uint32_t x) { return __builtin_popcount(x); }
 inline int ffs_(uint32_t x) { return __builtin_ffs(static_cast<int>(x)); }
 
@@ -228,6 +231,11 @@ RP_DEV T shfl_down(T v, int d) {
     return __shfl_down_sync(kFull, v, d);
 }
 RP_DEV uint32_t atomic_add(uint32_t* p, uint32_t v) { return atomicAdd(p, v); }
+template <typename T>
+RP_DEV void count_add(T* p, unsigned long long v) {
+    static_assert(sizeof(T) == sizeof(unsigned long long), "64-bit counter");
+    atomicAdd(reinterpret_cast<unsigned long long*>(p), v);
+}
 RP_DEV int popc(uint32_t x) { return __popc(x); }
 RP_DEV int ffs_(uint32_t x) { return __ffs(static_cast<int>(x)); }
 RP_DEV int16_t lo16(uint32_t a) { return static_cast<int16_t>(a & 0xffff); }
@@ -289,11 +297,7 @@ template <int G> RP_DEV bool any_converged_peer(bool p) { return ballot(p) != 0;
 template <int G> RP_DEV int glane() { return static_cast<int>(threadIdx.x & (G - 1)); }
 template <int G> RP_DEV uint32_t gbase() { return (threadIdx.x & 31u) & ~static_cast<uint32_t>(G - 1); }
 template <int G> RP_DEV uint32_t gmask() {
-#if defined(RP_EXPERIMENT_FULLMASK)
-    return kFull;   // experiment only: legal only while all groups of a warp follow the same control flow
-#else
     return G == 32 ? kFull : (((1u << (G & 31)) - 1u) << gbase<G>());
-#endif
 }
 template <int G> RP_DEV void gsync() { __syncwarp(gmask<G>()); }
 template <int G> RP_DEV uint32_t gballot(bool p) {

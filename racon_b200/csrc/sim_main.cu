@@ -50,45 +50,10 @@ void group_entry(void* arg) {
 
 extern "C" {
 
-/* Pairwise alignment through the simulated device code.  runs: n_pairs x run_stride uint32 ((count << 8) | op). */
-int rp_sim_aln(uint32_t n_pairs, const uint8_t* bases, const uint32_t* q_off, const uint32_t* q_len,
-               const uint32_t* t_off, const uint32_t* t_len, uint32_t max_len, uint32_t store_words, uint32_t* runs,
-               uint32_t run_stride, uint32_t* n_runs, int32_t* dist, uint32_t* status) {
-    rp::AlnParams P;
-    std::memset(&P, 0, sizeof(P));
-    P.n_pairs = n_pairs;
-    P.bases = bases;
-    P.q_off = q_off;
-    P.q_len = q_len;
-    P.t_off = t_off;
-    P.t_len = t_len;
-    std::vector<uint32_t> roff(n_pairs), rcap(n_pairs, run_stride);
-    for (uint32_t p = 0; p < n_pairs; ++p) roff[p] = p * run_stride;
-    P.runs = runs;
-    P.run_off = roff.data();
-    P.run_cap = rcap.data();
-    P.n_runs = n_runs;
-    P.dist = dist;
-    P.status = status;
-    P.lim.max_len = max_len;
-    P.lim.store_words = store_words;
-    P.lay = rp::make_aln_layout(P.lim);
-    std::vector<uint8_t> slot(P.lay.bytes + 64);
-    uint8_t* slot_al = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(slot.data()) + 15) & ~uintptr_t(15));
-    for (uint32_t p = 0; p < n_pairs; ++p) {
-        if (q_len[p] > max_len || t_len[p] > max_len) {
-            status[p] = rp::kAlnTooLong;
-            n_runs[p] = 0;
-            dist[p] = -1;
-            continue;
-        }
-        AlnJob job{&P, p, slot_al};
-        rp::sim::run_warp(aln_entry, &job);
-    }
-    return 0;
-}
-
-/* Same, plus breaking points: bp = n_pairs x bp_stride (t, q) points, n_bp = points per pair. */
+/* Pairwise alignment through the simulated device code.  runs: n_pairs x run_stride uint32 ((count << 8) | op).  A pair
+ * with a sequence longer than max_len gets status kAlnTooLong, no runs and distance -1.  With window_length != 0 also
+ * breaking points: bp = n_pairs x bp_stride (t, q) points, n_bp = points per pair; with 0, t_begin, q_start, bp and
+ * n_bp may be null. */
 int rp_sim_aln_bp(uint32_t n_pairs, const uint8_t* bases, const uint32_t* q_off, const uint32_t* q_len,
                   const uint32_t* t_off, const uint32_t* t_len, uint32_t max_len, uint32_t store_words, uint32_t* runs,
                   uint32_t run_stride, uint32_t* n_runs, int32_t* dist, uint32_t* status, uint32_t window_length,
@@ -125,42 +90,27 @@ int rp_sim_aln_bp(uint32_t n_pairs, const uint8_t* bases, const uint32_t* q_off,
     std::vector<uint8_t> slot(P.lay.bytes + 64);
     uint8_t* slot_al = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(slot.data()) + 15) & ~uintptr_t(15));
     for (uint32_t p = 0; p < n_pairs; ++p) {
+        if (q_len[p] > max_len || t_len[p] > max_len) {
+            status[p] = rp::kAlnTooLong;
+            n_runs[p] = 0;
+            dist[p] = -1;
+            continue;
+        }
         AlnJob job{&P, p, slot_al};
         rp::sim::run_warp(aln_entry, &job);
     }
     return 0;
 }
 
+/* The same without breaking points. */
+int rp_sim_aln(uint32_t n_pairs, const uint8_t* bases, const uint32_t* q_off, const uint32_t* q_len,
+               const uint32_t* t_off, const uint32_t* t_len, uint32_t max_len, uint32_t store_words, uint32_t* runs,
+               uint32_t run_stride, uint32_t* n_runs, int32_t* dist, uint32_t* status) {
+    return rp_sim_aln_bp(n_pairs, bases, q_off, q_len, t_off, t_len, max_len, store_words, runs, run_stride, n_runs, dist,
+                         status, 0, nullptr, nullptr, nullptr, 0, nullptr);
+}
+
 unsigned long rp_sim_leaf_pairs() { return rp::g_sim_leaf_pairs; }
-/* DP rows processed / rows that needed the full in-row carry scan (the rest took the one-shuffle short cut) */
-void rp_sim_scan_counts(unsigned long* out) {
-    out[0] = rp::g_sim_scan_rows;
-    out[1] = rp::g_sim_scan_full;
-}
-
-/* packing only (host-side cost of rp_poa_add_window): returns number of GPU windows packed */
-int rp_sim_pack_only(uint32_t n_windows, const char* bases, const char* quals, const uint64_t* seq_off,
-                     const uint8_t* seq_has_qual, const uint32_t* seq_begin, const uint32_t* seq_end,
-                     const uint32_t* win_first, const uint8_t* win_type, int trim) {
-    rp::PackedBatch pb(&kSimAlloc);
-    std::vector<const char*> sp, qp;
-    std::vector<uint32_t> ln;
-    for (uint32_t w = 0; w < n_windows; ++w) {
-        uint32_t s0 = win_first[w], s1 = win_first[w + 1];
-        sp.clear(); qp.clear(); ln.clear();
-        for (uint32_t s = s0; s < s1; ++s) {
-            sp.push_back(bases + seq_off[s]);
-            bool q = quals && seq_has_qual && seq_has_qual[s];
-            qp.push_back(q ? quals + seq_off[s] : nullptr);
-            ln.push_back(static_cast<uint32_t>(seq_off[s + 1] - seq_off[s]));
-        }
-        int r = pb.add(s1 - s0, sp.data(), ln.data(), qp.data(), seq_begin + s0, seq_end + s0, win_type[w], trim);
-        if (r != rp::kPackOk) return -100 + r;
-    }
-    pb.build_queue();
-    return static_cast<int>(pb.n_gpu());
-}
-
 /* Flat window set in, consensus out.  limits: {nmax, lmax, ki, ka, smem_per_group, tile_rows, debug_flags,
  * lanes per group (8/16/32), banded, band margin, matrix scratch cells (0 = nmax x padded lmax), columns per lane
  * of a banded row (16/8/4; 8 and 4 only with 32 lanes)}.  With banded,

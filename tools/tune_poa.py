@@ -1,6 +1,7 @@
-"""Kernel-only throughput of rp_poa_kernel over its launch-shape knobs (lanes per window, blocks per SM, banded),
-inputs resident in HBM, CUDA-event timed.  A tuning aid; bench.py is the judged measurement.
-  python tools/tune_poa.py [--windows 10000] [--configs "banded,lanes,blocks_per_sm[,band columns per lane];..."]"""
+"""Kernel-only throughput of rp_poa_kernel over its layouts (lanes per window, band columns per lane, banded), inputs
+resident in HBM, CUDA-event timed.  A tuning aid; bench.py is the judged measurement.  Blocks per SM are a function of the
+layout (poa_blocks_per_sm in racon_b200/csrc/rp_api.cu): re-tuning them means editing that function and rebuilding.
+  python tools/tune_poa.py [--windows 10000] [--configs "banded,lanes[,band columns per lane];..."]"""
 import argparse
 import json
 import os
@@ -13,7 +14,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--windows", type=int, default=10000)
     ap.add_argument("--reps", type=int, default=3)
-    ap.add_argument("--configs", default="0,32,4;0,16,4;0,8,4;1,16,4;1,8,4;1,8,3;1,8,2;0,8,3;0,16,3;1,16,3")
+    ap.add_argument("--configs", default="0,32;0,16;0,8;1,16;1,8")
     ap.add_argument("--two-streams", action="store_true", help="also time launches alternating between two objects")
     ap.add_argument("--wlen", type=int, default=500, help="window length of the synthetic windows")
     ap.add_argument("--replicate", type=int, default=1, help="every window this many times in a row (lock-step experiment)")
@@ -28,10 +29,9 @@ def main():
     ref = None
     for cfg in args.configs.split(";"):
         f = [int(x) for x in cfg.split(",")]
-        banded, g, bps = f[:3]
-        k = f[3] if len(f) > 3 else 16
+        banded, g = f[:2]
+        k = f[2] if len(f) > 2 else 16
         os.environ["RP_POA_GROUP"] = str(g)
-        os.environ["RP_BLOCKS_PER_SM"] = str(bps)
         os.environ["RP_POA_BAND_K"] = str(k)
         try:
             b = api.PoaBatch(device=0, window_length=args.wlen, banded=bool(banded), mem_bytes=int(30e9))
@@ -57,7 +57,7 @@ def main():
             torch.cuda.synchronize()
             ms = [ev[kk].elapsed_time(ev[kk + 1]) for kk in range(args.reps)]
             info = b.info()
-            res = {"banded": banded, "lanes": g, "blocks_per_sm": bps, "band_cols_per_lane": k, "ms": [round(x, 2) for x in ms],
+            res = {"banded": banded, "lanes": g, "band_cols_per_lane": k, "ms": [round(x, 2) for x in ms],
                    "windows_per_s": round(ws.n_windows / (min(ms) * 1e-3)), "workers": info["workers"],
                    "scratch_MB_per_worker": round(info["scratch_bytes_per_worker"] / 1e6, 2),
                    "bad_status": int((status != 0).sum()), "fnv200": ck, "same_as_first": full == ref,
@@ -84,7 +84,7 @@ def main():
                 b2.close()
             b.close()
         except Exception as e:  # noqa: BLE001
-            res = {"banded": banded, "lanes": g, "blocks_per_sm": bps, "error": str(e)[:300]}
+            res = {"banded": banded, "lanes": g, "error": str(e)[:300]}
         print(json.dumps(res), flush=True)
 
 
