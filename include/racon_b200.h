@@ -38,7 +38,8 @@ enum {
 /* per-window soft status reported by rp_poa_window_status (0 = consensus produced on the GPU) */
 enum {
     RP_WIN_OK = 0,
-    RP_WIN_NODE_LIMIT = 1,
+    RP_WIN_NODE_LIMIT = 1,       /* the graph outgrew the escalation pass's node budget: 8 x (6 * window_len_hint + 64)
+                                    nodes, at most 65 000 (the first pass holds 6 * window_len_hint + 64) */
     RP_WIN_EDGE_LIMIT = 2,
     RP_WIN_ALIGNED_LIMIT = 3,
     RP_WIN_NEEDS_INT32 = 4,      /* the score matrix may leave int16 (|gap| > 64, |gap| * (graph depth + length) > ~31k, or

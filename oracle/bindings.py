@@ -56,6 +56,9 @@ def oracle_lib():
             lib.oracle_myers_cigar.restype = C.c_int64
             lib.oracle_myers_cigar.argtypes = [C.c_char_p, C.c_uint32, C.c_char_p, C.c_uint32, C.c_void_p,
                                                C.c_uint64, C.c_void_p]
+        lib.oracle_graph_shape.restype = C.c_int
+        lib.oracle_graph_shape.argtypes = _CONS_ARGS[:13] + [C.c_uint32, C.c_void_p, C.c_uint32] + [C.c_void_p, C.c_uint32] + \
+            [C.c_void_p] * 3
         lib.oracle_poa_trace_begin.restype = None
         lib.oracle_poa_trace_begin.argtypes = []
         lib.oracle_poa_trace_end.restype = C.c_uint64
@@ -129,6 +132,26 @@ def oracle_matrix_ranges(ws, m=3, x=-5, g=-4, window_length=500, trim=True):
             n = lib.oracle_poa_trace_end(rec.ctypes.data, cap)
         out.append(rec[:min(n, cap)])
     return out
+
+
+def oracle_graph_shape(ws, m=3, x=-5, g=-4, window_length=500, threads=1):
+    """Per window, (nodes, max in-degree, max aligned-set size) of the oracle's graph: nodes = uint32 array of the node
+    count after the backbone and after each aligned layer, in the order the oracle aligned its layers (sorted by begin;
+    empty for windows of fewer than 3 sequences); the two maxima are those of the final graph."""
+    n = ws.n_windows
+    stride = max(16, _max_nodes_bound(ws))
+    out = np.zeros((n, stride), dtype=np.uint8)
+    per_win = np.diff(ws.win_first.astype(np.int64))
+    nstride = max(1, int(per_win.max()) if n else 1)
+    nodes = np.zeros((n, nstride), np.uint32)
+    n_nodes, indeg, aligned = (np.zeros(n, np.uint32) for _ in range(3))
+    r = oracle_lib().oracle_graph_shape(n, _ptr(ws.bases), _ptr(ws.quals), _ptr(ws.seq_off), _ptr(ws.seq_has_qual),
+                                        _ptr(ws.seq_begin), _ptr(ws.seq_end), _ptr(ws.win_first), _ptr(ws.win_type),
+                                        m, x, g, window_length, threads, out.ctypes.data, stride, nodes.ctypes.data,
+                                        nstride, n_nodes.ctypes.data, indeg.ctypes.data, aligned.ctypes.data)
+    if r != 0:
+        raise RuntimeError("oracle graph shape failed (%d)" % r)
+    return [(nodes[w, :n_nodes[w]].copy(), int(indeg[w]), int(aligned[w])) for w in range(n)]
 
 
 def ref_edlib_cigar(q, t):

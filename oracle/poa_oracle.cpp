@@ -460,16 +460,25 @@ std::vector<uint32_t> weights_of(const Seq& s) {  // graph.cpp:121-146
     return w;
 }
 
+/* The graph's shape, for oracle_graph_shape: node count after the backbone and after each layer (in the order the
+ * layers are aligned), and the largest in-degree and aligned-set size of the final graph. */
+struct Shape {
+    std::vector<uint32_t> nodes;
+    uint32_t max_indeg = 0, max_aligned = 0;
+};
+
 // Window::generate_consensus, window.cpp:65-149.  seqs[0] = backbone.
 bool window_consensus(const std::vector<Seq>& seqs, int type_tgs, bool trim, Engine& engine, std::string* consensus,
-                      std::vector<uint32_t>* coverage) {
+                      std::vector<uint32_t>* coverage, Shape* shape = nullptr) {
     coverage->clear();
+    if (shape) *shape = Shape{};
     if (seqs.size() < 3) {
         consensus->assign(seqs[0].data, seqs[0].len);
         return false;
     }
     Graph graph;
     graph.add_alignment({}, seqs[0].data, seqs[0].len, weights_of(seqs[0]));
+    if (shape) shape->nodes.push_back(graph.size());
 
     std::vector<uint32_t> rank(seqs.size());
     for (uint32_t i = 0; i < seqs.size(); ++i) rank[i] = i;
@@ -491,6 +500,7 @@ bool window_consensus(const std::vector<Seq>& seqs, int type_tgs, bool trim, Eng
                 if (it.first != -1) it.first = static_cast<int32_t>(map[it.first]);  // graph.cpp:597-605
         }
         graph.add_alignment(alignment, s.data, s.len, weights_of(s));
+        if (shape) shape->nodes.push_back(graph.size());
     }
     {
         uint64_t n = graph.size(), mi = 0, ma = 0;
@@ -504,6 +514,10 @@ bool window_consensus(const std::vector<Seq>& seqs, int type_tgs, bool trim, Eng
         while (cur < mi && !g_stats.max_indeg.compare_exchange_weak(cur, mi)) {}
         cur = g_stats.max_aligned.load();
         while (cur < ma && !g_stats.max_aligned.compare_exchange_weak(cur, ma)) {}
+        if (shape) {
+            shape->max_indeg = static_cast<uint32_t>(mi);
+            shape->max_aligned = static_cast<uint32_t>(ma);
+        }
     }
 
     std::vector<uint32_t> cov;
@@ -524,18 +538,12 @@ bool window_consensus(const std::vector<Seq>& seqs, int type_tgs, bool trim, Eng
     return true;
 }
 
-}  // namespace
-
-extern "C" {
-
-/* Same contract as ref_poa_consensus (oracle/ref_harness.cpp) plus an optional per-base coverage
- * matrix `cov_out` (n_windows x out_stride uint32, coverage of the returned consensus). */
-double oracle_poa_consensus(uint32_t n_windows, const char* bases, const char* quals, const uint64_t* seq_off,
-                            const uint8_t* seq_has_qual, const uint32_t* seq_begin, const uint32_t* seq_end,
-                            const uint32_t* win_first, const uint8_t* win_type, int8_t match, int8_t mismatch,
-                            int8_t gap, uint32_t window_length, int trim, uint32_t n_threads, char* out,
-                            uint32_t out_stride, uint32_t* out_len, uint8_t* polished, uint32_t* cov_out) {
-    (void)window_length;
+/* oracle_poa_consensus, and with `shape_out` also each window's Shape (see oracle_graph_shape) */
+double run_windows(uint32_t n_windows, const char* bases, const char* quals, const uint64_t* seq_off,
+                   const uint8_t* seq_has_qual, const uint32_t* seq_begin, const uint32_t* seq_end,
+                   const uint32_t* win_first, const uint8_t* win_type, int8_t match, int8_t mismatch, int8_t gap,
+                   int trim, uint32_t n_threads, char* out, uint32_t out_stride, uint32_t* out_len, uint8_t* polished,
+                   uint32_t* cov_out, std::vector<Shape>* shape_out) {
     if (n_threads == 0) n_threads = 1;
     std::atomic<uint32_t> next(0);
     std::atomic<int> failed(0);
@@ -567,7 +575,8 @@ double oracle_poa_consensus(uint32_t n_windows, const char* bases, const char* q
             }
             std::string cons;
             std::vector<uint32_t> cov;
-            bool ok = window_consensus(seqs, win_type[w], trim != 0, engine, &cons, &cov);
+            bool ok = window_consensus(seqs, win_type[w], trim != 0, engine, &cons, &cov,
+                                       shape_out ? &(*shape_out)[w] : nullptr);
             if (cons.size() > out_stride) {
                 failed = 1;
                 continue;
@@ -589,6 +598,51 @@ double oracle_poa_consensus(uint32_t n_windows, const char* bases, const char* q
     auto t1 = std::chrono::steady_clock::now();
     if (failed) return -1.0;
     return std::chrono::duration<double>(t1 - t0).count();
+}
+
+}  // namespace
+
+extern "C" {
+
+/* Same contract as ref_poa_consensus (oracle/ref_harness.cpp) plus an optional per-base coverage
+ * matrix `cov_out` (n_windows x out_stride uint32, coverage of the returned consensus). */
+double oracle_poa_consensus(uint32_t n_windows, const char* bases, const char* quals, const uint64_t* seq_off,
+                            const uint8_t* seq_has_qual, const uint32_t* seq_begin, const uint32_t* seq_end,
+                            const uint32_t* win_first, const uint8_t* win_type, int8_t match, int8_t mismatch,
+                            int8_t gap, uint32_t window_length, int trim, uint32_t n_threads, char* out,
+                            uint32_t out_stride, uint32_t* out_len, uint8_t* polished, uint32_t* cov_out) {
+    (void)window_length;
+    return run_windows(n_windows, bases, quals, seq_off, seq_has_qual, seq_begin, seq_end, win_first, win_type, match,
+                       mismatch, gap, trim, n_threads, out, out_stride, out_len, polished, cov_out, nullptr);
+}
+
+/* The consensus pass of oracle_poa_consensus, reporting each window's graph shape instead of its consensus:
+ * nodes = n_windows x nodes_stride uint32, the node count after the backbone and after each aligned layer, in the
+ * order the layers are aligned (sorted by begin; layers skipped as empty are not counted), n_nodes = entries per
+ * window (0 for windows of fewer than 3 sequences, which build no graph), max_indeg / max_aligned = the largest
+ * in-degree and aligned-set size of the final graph.  Returns 0, or -1 when an output does not fit. */
+int oracle_graph_shape(uint32_t n_windows, const char* bases, const char* quals, const uint64_t* seq_off,
+                       const uint8_t* seq_has_qual, const uint32_t* seq_begin, const uint32_t* seq_end,
+                       const uint32_t* win_first, const uint8_t* win_type, int8_t match, int8_t mismatch, int8_t gap,
+                       uint32_t window_length, uint32_t n_threads, char* out, uint32_t out_stride, uint32_t* nodes,
+                       uint32_t nodes_stride, uint32_t* n_nodes, uint32_t* max_indeg, uint32_t* max_aligned) {
+    (void)window_length;
+    std::vector<uint32_t> out_len(n_windows);
+    std::vector<uint8_t> polished(n_windows);
+    std::vector<Shape> shapes(n_windows);
+    if (run_windows(n_windows, bases, quals, seq_off, seq_has_qual, seq_begin, seq_end, win_first, win_type, match,
+                    mismatch, gap, 1, n_threads, out, out_stride, out_len.data(), polished.data(), nullptr,
+                    &shapes) < 0)
+        return -1;
+    for (uint32_t w = 0; w < n_windows; ++w) {
+        const Shape& s = shapes[w];
+        if (s.nodes.size() > nodes_stride) return -1;
+        std::copy(s.nodes.begin(), s.nodes.end(), nodes + static_cast<uint64_t>(w) * nodes_stride);
+        n_nodes[w] = static_cast<uint32_t>(s.nodes.size());
+        max_indeg[w] = s.max_indeg;
+        max_aligned[w] = s.max_aligned;
+    }
+    return 0;
 }
 
 /* out[12]: alignments, cells, pred_cells, sink_ties, multi_sink, subgraph_alignments, branch_completions,

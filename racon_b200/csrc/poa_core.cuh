@@ -68,7 +68,7 @@ struct PoaLimits {
 struct SlotLayout {
     uint64_t code, flags, in_cnt, al_cnt, cov, in_tail, in_w, al, order_a, order_b, rank_of, dp_order, dp_rank,
         rec, pred_ovf, H, aln, cur, member, has_out_sub, score, cpred, sorder, srank, marks, stack,
-        newlist, ccarry, bpos, bs, bytes;
+        newlist, ccarry, bpos, bs, delta, bytes;
 };
 
 RP_HD uint64_t align_up(uint64_t x, uint64_t a) { return (x + a - 1) / a * a; }
@@ -112,6 +112,7 @@ RP_HD SlotLayout make_layout(const PoaLimits& L) {
     s.ccarry = take((n + 2) * 2 * 2);
     s.bpos = take(n * 2);
     s.bs = take(n + 2 + 64);
+    s.delta = take((n + 4) * 2);
     s.bytes = align_up(o, 4096);
     return s;
 }
@@ -1689,11 +1690,62 @@ struct PoaWarp {
         return true;
     }
 
+    /* add_alignment, Phase D (below): the order update's counters and the remap */
+    template <bool kSmem>
+    RP_DEV void merge_order(uint32_t n_old, uint32_t n_new) {
+        /* (the slot's base is not kept: one more member of this struct costs per-window spills) */
+        uint16_t* delta = kSmem ? reinterpret_cast<uint16_t*>(smem)
+                                : reinterpret_cast<uint16_t*>(bs + (P->lay.delta - P->lay.bs));
+        for (uint32_t q = lane; q < n_old + 2; q += G) delta[q] = 0;
+        syncwarp();
+        for (uint32_t k = lane; k < n_new; k += G) {
+            uint32_t j = newlist[k] >> 16;
+            uint32_t key = aln[j];  // aligned new node: end of its cluster block; insertion: K_{j-1}
+            uint32_t id = n_old + k;
+            uint32_t nr = key + 1 + k;
+            order_nxt[nr] = static_cast<uint16_t>(id);
+            rank_of[id] = static_cast<uint16_t>(nr);
+#if defined(RP_HOST_SIM)
+            delta[key + 1] = static_cast<uint16_t>(delta[key + 1] + 1);
+#else
+            atomicAdd(reinterpret_cast<unsigned int*>(delta + ((key + 1) & ~1u)), (key + 1) & 1u ? 0x10000u : 1u);
+#endif
+        }
+        syncwarp();
+        /* inclusive prefix of the counters, then a remap pass whose HBM loads are batched */
+        uint32_t carry = 0;
+        for (uint32_t q0 = 1; q0 <= n_old; q0 += G) {
+            uint32_t q = q0 + lane;
+            uint32_t d = q <= n_old ? delta[q] : 0;
+            uint32_t inc = warp_incl_sum(d) + carry;
+            if (q <= n_old) delta[q] = static_cast<uint16_t>(inc);
+            carry = shfl(inc, G - 1);
+        }
+        syncwarp();
+        constexpr int kV = 8;
+        for (uint32_t q0 = 1; q0 <= n_old; q0 += G * kV) {
+            uint32_t v[kV];
+#pragma unroll
+            for (int u = 0; u < kV; ++u) {
+                uint32_t q = q0 + u * G + lane;
+                v[u] = q <= n_old ? order[q] : 0;
+            }
+#pragma unroll
+            for (int u = 0; u < kV; ++u) {
+                uint32_t q = q0 + u * G + lane;
+                if (q <= n_old) {
+                    uint32_t nr = q + delta[q];
+                    order_nxt[nr] = static_cast<uint16_t>(v[u]);
+                    rank_of[v[u]] = static_cast<uint16_t>(nr);
+                }
+            }
+        }
+    }
+
     /* ---------------------------------------------------------------- graph merge (graph.cpp:155-247) +
      * incremental order update.  aln[j] = aligned node or kNone for every read position j. */
     RP_DEV void add_alignment(const uint8_t* seq, const uint8_t* w, uint32_t len, uint32_t b0) {
         const uint32_t n_old = N;
-        uint16_t* delta = reinterpret_cast<uint16_t*>(smem);  // n_old + 2 counters (ring is idle now)
         /* All phases handle kU positions per lane at a time with the loads of one dependency level issued
          * together (the graph is in HBM: every level costs a full memory latency). */
         constexpr int kU = 4;
@@ -1890,54 +1942,13 @@ struct PoaWarp {
         /* Phase D: merge new nodes into the processing order.  New node k (read order) with key K goes to
          * rank K + 1 + k; an old node at rank q moves to q + #{new nodes with key < q}. */
         if (n_new > 0) {
-            if ((n_old + 4) * 2 > smem_bytes) {
-                fail(kWinNodeLimit);
-                return;
-            }
-            for (uint32_t q = lane; q < n_old + 2; q += G) delta[q] = 0;
-            syncwarp();
-            for (uint32_t k = lane; k < n_new; k += G) {
-                uint32_t j = newlist[k] >> 16;
-                uint32_t key = aln[j];  // aligned new node: end of its cluster block; insertion: K_{j-1}
-                uint32_t id = n_old + k;
-                uint32_t nr = key + 1 + k;
-                order_nxt[nr] = static_cast<uint16_t>(id);
-                rank_of[id] = static_cast<uint16_t>(nr);
-#if defined(RP_HOST_SIM)
-                delta[key + 1] = static_cast<uint16_t>(delta[key + 1] + 1);
-#else
-                atomicAdd(reinterpret_cast<unsigned int*>(delta + ((key + 1) & ~1u)), (key + 1) & 1u ? 0x10000u : 1u);
-#endif
-            }
-            syncwarp();
-            /* inclusive prefix of the counters in shared memory, then a remap pass whose HBM loads are batched */
-            uint32_t carry = 0;
-            for (uint32_t q0 = 1; q0 <= n_old; q0 += G) {
-                uint32_t q = q0 + lane;
-                uint32_t d = q <= n_old ? delta[q] : 0;
-                uint32_t inc = warp_incl_sum(d) + carry;
-                if (q <= n_old) delta[q] = static_cast<uint16_t>(inc);
-                carry = shfl(inc, G - 1);
-            }
-            syncwarp();
-            constexpr int kV = 8;
-            for (uint32_t q0 = 1; q0 <= n_old; q0 += G * kV) {
-                uint32_t v[kV];
-#pragma unroll
-                for (int u = 0; u < kV; ++u) {
-                    uint32_t q = q0 + u * G + lane;
-                    v[u] = q <= n_old ? order[q] : 0;
-                }
-#pragma unroll
-                for (int u = 0; u < kV; ++u) {
-                    uint32_t q = q0 + u * G + lane;
-                    if (q <= n_old) {
-                        uint32_t nr = q + delta[q];
-                        order_nxt[nr] = static_cast<uint16_t>(v[u]);
-                        rank_of[v[u]] = static_cast<uint16_t>(nr);
-                    }
-                }
-            }
+            /* its n_old + 2 counters live in shared memory (the ring is idle now) when they fit, else in the slot's HBM
+             * copy, so that nmax is the only node limit whatever the group's share of shared memory; one instantiation
+             * per memory space, so that every access compiles to a shared- or a global-memory instruction */
+            if ((n_old + 4) * 2 <= smem_bytes)
+                merge_order<true>(n_old, n_new);
+            else
+                merge_order<false>(n_old, n_new);
             if (lane == 0) order_nxt[0] = kNone;
             uint16_t* t = order;
             order = order_nxt;

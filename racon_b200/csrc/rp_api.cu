@@ -998,8 +998,9 @@ rp_status rp_poa_run(rp_poa* p) {
 }
 
 /* Windows whose graph outgrew the default per-window limits (very deep coverage, very long layers) are run
- * again ON THE GPU with 8x the node budget, 4x the layer length and 96 in-edge slots, on a smaller set of
- * workers (the reference hands such windows to the CPU, cudapolisher.cpp:354-370; this library has no CPU path). */
+ * again ON THE GPU with 8x the node budget (lim_big.nmax, the only node limit of this pass in every layout: add_alignment
+ * keeps its order counters in HBM when the group's shared memory is too small), 4x the layer length and 96 in-edge
+ * slots, on a smaller set of workers (the reference hands such windows to the CPU, cudapolisher.cpp:354-370; this library has no CPU path). */
 static rp_status escalate(rp_poa* p) {
     const uint32_t n = p->P.n_windows;
     std::vector<uint32_t> redo;
