@@ -55,7 +55,10 @@ def oracle_lib():
         if hasattr(lib, "oracle_myers_cigar"):
             lib.oracle_myers_cigar.restype = C.c_int64
             lib.oracle_myers_cigar.argtypes = [C.c_char_p, C.c_uint32, C.c_char_p, C.c_uint32, C.c_void_p,
-                                               C.c_uint64, C.c_void_p]
+                                               C.c_uint64, C.c_void_p, C.c_uint64]
+            lib.oracle_myers_tree.restype = C.c_int64
+            lib.oracle_myers_tree.argtypes = [C.c_char_p, C.c_uint32, C.c_char_p, C.c_uint32, C.c_uint64, C.c_void_p,
+                                              C.c_uint64]
         lib.oracle_graph_shape.restype = C.c_int
         lib.oracle_graph_shape.argtypes = _CONS_ARGS[:13] + [C.c_uint32, C.c_void_p, C.c_uint32] + [C.c_void_p, C.c_uint32] + \
             [C.c_void_p] * 3
@@ -164,14 +167,35 @@ def ref_edlib_cigar(q, t):
     return buf.raw[:n].decode(), ed.value
 
 
-def oracle_myers_cigar(q, t):
+EDLIB_RULE = 1 << 20   # edlib traces a node back below this many bytes of alignment data, and splits it above
+
+
+def edlib_data_bytes(ql, tl):
+    """The alignment data edlib's rule weighs for a (ql x tl) node (edlib.cpp:1155-1157)."""
+    return 20 * ((ql + 63) // 64) * tl + 8 * tl
+
+
+def oracle_myers_cigar(q, t, rule=EDLIB_RULE):
+    """(CIGAR, edit distance) edlib returns, restated; with another `rule` (bytes), what it would return if its 1 MiB
+    rule were moved there."""
     cap = 4 * (len(q) + len(t)) + 64
     buf = C.create_string_buffer(cap)
     ed = C.c_int32(0)
-    n = oracle_lib().oracle_myers_cigar(q, len(q), t, len(t), buf, cap, C.byref(ed))
+    n = oracle_lib().oracle_myers_cigar(q, len(q), t, len(t), buf, cap, C.byref(ed), rule)
     if n < 0:
         raise RuntimeError("oracle myers failed (%d)" % n)
     return buf.raw[:n].decode(), ed.value
+
+
+def oracle_myers_tree(q, t, rule=EDLIB_RULE):
+    """edlib's node tree for the pair: an (nodes, 4) int64 array of (query length, target length, score, leaf) in
+    pre-order, leaf = 1 for a traceback node and 0 for a Hirschberg split; nodes with an empty side are left out."""
+    cap = 2 * (len(q) + len(t)) + 8
+    out = np.zeros((cap, 4), np.int32)
+    n = oracle_lib().oracle_myers_tree(q, len(q), t, len(t), rule, out.ctypes.data, cap)
+    if n < 0:
+        raise RuntimeError("oracle myers tree failed (%d)" % n)
+    return out[:n].astype(np.int64)
 
 
 def oracle_breaking_points(cigar, t_begin, t_end, q_start, window_length):

@@ -21,7 +21,8 @@
  *
  * PINNING: tests/test_myers_oracle.py compares this file with the UNMODIFIED edlib (oracle/_ref, ref_edlib_cigar)
  * on random pairs across lengths (1 .. 6000, i.e. both the traceback and the Hirschberg regime), error rates and
- * length imbalances, byte for byte.
+ * length imbalances, and on tie-rich pairs (homopolymer-length errors, tandem repeats, low-complexity runs) in both
+ * regimes, byte for byte.
  */
 #include <algorithm>
 #include <cstdint>
@@ -83,14 +84,21 @@ void traceback(const char* q, int n, const char* t, int m, std::string& ops) {
     ops.append(rev.rbegin(), rev.rend());
 }
 
-void obtain_alignment(const char* q, int n, const char* t, int m, int best, std::string& ops) {
+/* rule: the alignment-data size (bytes) from which on edlib switches from the traceback to Hirschberg; edlib's is
+ * 1 MiB, tests move it to show that a pair's alignment depends on which side of the rule a node falls.
+ * tree (optional): receives (query length, target length, score, leaf) of every node with a non-empty query and
+ * target, in pre-order (a node, then its left part, then its right part). */
+void obtain_alignment(const char* q, int n, const char* t, int m, int best, long long rule, std::string& ops,
+                      std::vector<int32_t>* tree) {
     if (n == 0 || m == 0) {  // edlib.cpp:1136-1143
         ops.append(static_cast<size_t>(n + m), n == 0 ? 'D' : 'I');
         return;
     }
     const long long blocks = (n + 63) / 64;
     const long long data = (2 * 8 + 4) * blocks * m + 2LL * 4 * m;  // edlib.cpp:1155-1157
-    if (data < 1024 * 1024) {
+    const bool leaf = data < rule;
+    if (tree) tree->insert(tree->end(), {n, m, best, leaf ? 1 : 0});
+    if (leaf) {
         traceback(q, n, t, m, ops);
         return;
     }
@@ -126,24 +134,29 @@ void obtain_alignment(const char* q, int n, const char* t, int m, int best, std:
         return;
     }
     const int ul = split + 1;
-    obtain_alignment(q, ul, t, lw, ls, ops);
-    obtain_alignment(q + ul, n - ul, t + lw, rw, rs, ops);
+    obtain_alignment(q, ul, t, lw, ls, rule, ops, tree);
+    obtain_alignment(q + ul, n - ul, t + lw, rw, rs, rule, ops, tree);
+}
+
+int edit_distance_of(const char* q, uint32_t ql, const char* t, uint32_t tl) {
+    std::vector<int> col;
+    last_column(q, static_cast<int>(ql), t, static_cast<int>(tl), col);
+    return col[ql];
 }
 
 }  // namespace
 
 extern "C" {
 
-/* CIGAR (standard format) of the alignment edlib would return for (query, target); returns its length,
- * -2 if `cap` is too small.  *edit_distance receives the NW edit distance. */
+/* CIGAR (standard format) of the alignment edlib would return for (query, target) if its 1 MiB rule were `rule`
+ * bytes (edlib: 1048576); returns its length, -2 if `cap` is too small.  *edit_distance receives the NW edit
+ * distance. */
 int64_t oracle_myers_cigar(const char* q, uint32_t ql, const char* t, uint32_t tl, char* out, uint64_t cap,
-                           int32_t* edit_distance) {
-    std::vector<int> col;
-    last_column(q, static_cast<int>(ql), t, static_cast<int>(tl), col);
-    const int best = col[ql];
+                           int32_t* edit_distance, uint64_t rule) {
+    const int best = edit_distance_of(q, ql, t, tl);
     if (edit_distance) *edit_distance = best;
     std::string ops;
-    obtain_alignment(q, static_cast<int>(ql), t, static_cast<int>(tl), best, ops);
+    obtain_alignment(q, static_cast<int>(ql), t, static_cast<int>(tl), best, static_cast<long long>(rule), ops, nullptr);
     std::string cigar;
     for (size_t i = 0; i < ops.size();) {
         size_t j = i;
@@ -155,6 +168,21 @@ int64_t oracle_myers_cigar(const char* q, uint32_t ql, const char* t, uint32_t t
     if (cigar.size() + 1 > cap) return -2;
     std::memcpy(out, cigar.c_str(), cigar.size() + 1);
     return static_cast<int64_t>(cigar.size());
+}
+
+/* The node tree of the same alignment: 4 int32 per node (query length, target length, score, 1 for a traceback leaf /
+ * 0 for a Hirschberg split), pre-order, nodes with an empty side left out.  Returns the node count, -2 if more than
+ * `cap` nodes. */
+int64_t oracle_myers_tree(const char* q, uint32_t ql, const char* t, uint32_t tl, uint64_t rule, int32_t* out,
+                          uint64_t cap) {
+    const int best = edit_distance_of(q, ql, t, tl);
+    std::string ops;
+    std::vector<int32_t> tree;
+    obtain_alignment(q, static_cast<int>(ql), t, static_cast<int>(tl), best, static_cast<long long>(rule), ops, &tree);
+    const uint64_t nodes = tree.size() / 4;
+    if (nodes > cap) return -2;
+    if (!tree.empty()) std::memcpy(out, tree.data(), tree.size() * sizeof(int32_t));
+    return static_cast<int64_t>(nodes);
 }
 
 }  // extern "C"

@@ -32,6 +32,8 @@ def main():
         edlib["hirschberg/%d" % n] = [util.cigar_answer(ob.ref_edlib_cigar(q, t))
                                       for q, t in tm.hirschberg_pairs(n, err, count)]
     edlib["degenerate"] = [util.cigar_answer(ob.ref_edlib_cigar(q, t)) for q, t in tm.DEGENERATE]
+    for n in tm.TIES_TRACEBACK + tm.TIES_HIRSCHBERG:
+        edlib["ties/%d" % n] = [util.cigar_answer(ob.ref_edlib_cigar(q, t)) for q, t in tm.tie_pairs(n)]
     with open(os.path.join(ROOT, "tests", "golden", "ref_answers.json"), "w") as f:
         json.dump({"source": "oracle/_ref (the unmodified reference)", "poa": poa, "edlib": edlib}, f,
                   separators=(",", ":"))

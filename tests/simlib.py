@@ -61,8 +61,9 @@ def runs_to_cigar(runs):
     return "".join("%d%s" % (int(r) >> 8, chr(int(r) & 0xff)) for r in runs)
 
 
-def sim_align(pairs, max_len=None, store_words=53000):
-    """pairs: [(query bytes, target bytes), ...] -> ([(cigar, distance)], status array)"""
+def sim_align(pairs, max_len=None, store_words=53000, run_stride=None):
+    """pairs: [(query bytes, target bytes), ...] -> ([(cigar, distance)], status array).  run_stride: the run capacity
+    of every pair (default 2 * max_len + 8, more than any CIGAR needs)."""
     n = len(pairs)
     blob = b"".join(q + t for q, t in pairs)
     bases = np.frombuffer(blob, dtype=np.uint8).copy() if blob else np.zeros(1, np.uint8)
@@ -78,7 +79,7 @@ def sim_align(pairs, max_len=None, store_words=53000):
         o += len(t)
     if max_len is None:
         max_len = int(max([1] + [max(len(q), len(t)) for q, t in pairs]))
-    stride = 2 * max_len + 8
+    stride = run_stride or 2 * max_len + 8
     runs = np.zeros((n, stride), np.uint32)
     n_runs = np.zeros(n, np.uint32)
     dist = np.zeros(n, np.int32)
