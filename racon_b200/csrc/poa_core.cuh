@@ -15,7 +15,7 @@
  *     lane-strided data-parallel loop, so HBM latency is overlapped 32-wide.
  *   * The DP keeps a whole 512-column row chunk in registers: lane l owns 16 consecutive columns as
  *     8 packed int16x2 registers; predecessor rows come from a shared-memory ring of the most recent
- *     rows (conflict-free swizzled 128-bit loads) or, for far predecessors, from the HBM copy; the cell
+ *     rows (conflict-free 128-bit loads) or, for far predecessors, from the HBM copy; the cell
  *     update is two DPX VIADDMNMX.S16x2 per predecessor per register; the in-row gap recurrence is a
  *     lane-local max-plus chain plus a 5-step warp shuffle scan.
  *   * Rows are processed in an incrementally maintained topological order (aligned clusters kept
@@ -122,8 +122,8 @@ struct PoaParams {
     int32_t match, mismatch, gap;
     /* per-register constants of a full-matrix DP row, derived from `gap` by set_scores(): [r] = (0, (r+1)g) bridge
      * offsets, [8+r] = ((r+1)g, (r+9)g) carry offsets, [16] = (g, g).  Kept in the parameter block so that the row loop
-     * takes them straight from the constant bank as instruction operands — as loop-invariant registers they do not
-     * survive the kernel's register cap and were rebuilt (about 35 instructions) in every row. */
+     * reads the sixteen offsets from the constant bank (one LDC each) — as loop-invariant registers they do not fit the
+     * kernel's register budget and were rebuilt (about 35 instructions) in every row.  (g, g) is held in a register. */
     uint32_t row_consts[17];
     uint32_t n_windows;
     /* inputs, packed by the host in processing order (backbone first, layers sorted as window.cpp:85-86) */
@@ -178,13 +178,13 @@ inline void set_scores(PoaParams& P, int32_t match, int32_t mismatch, int32_t ga
  * column r in its low half and column 8+r in its high half, so the in-row gap recurrence runs as two
  * packed 8-long chains and the diagonal operand of register r is simply register r-1 of the predecessor.
  * perm(): logical column -> element index in a row stored in that register order (HBM copy);
- * swz(): additionally XOR-swizzles 16-byte granules so the two LDS.128 of a lane are bank-conflict free. */
+ * swz_e(): additionally XOR-swizzles 16-byte granules so the two LDS.128 of a lane are bank-conflict free (band rows;
+ * the full-matrix rows in shared memory have a layout of their own, PoaWarp::smem_elem). */
 RP_DEV uint32_t perm(uint32_t c) { return (c & ~15u) | ((c & 7u) << 1) | ((c >> 3) & 1u); }
 RP_DEV uint32_t swz_e(uint32_t e) {
     uint32_t q = e >> 3;
     return ((q ^ ((q >> 3) & 1u)) << 3) | (e & 7u);
 }
-RP_DEV uint32_t swz(uint32_t c) { return swz_e(perm(c)); }
 
 struct Row8 {
     uint32_t r[8];
@@ -218,20 +218,6 @@ RP_DEV Row8 load_row_smem(const int16_t* row, int lane) {
     o.r[0] = a.x; o.r[1] = a.y; o.r[2] = a.z; o.r[3] = a.w;
     o.r[4] = c.x; o.r[5] = c.y; o.r[6] = c.z; o.r[7] = c.w;
     return o;
-}
-/* the same with the lane's two (swizzled) granule indices handed in: dp() derives them once per alignment */
-RP_DEV Row8 load_row_smem_at(const int16_t* row, uint32_t p0, uint32_t p1) {
-    const U4* b = reinterpret_cast<const U4*>(row);
-    U4 a = b[p0], c = b[p1];
-    Row8 o;
-    o.r[0] = a.x; o.r[1] = a.y; o.r[2] = a.z; o.r[3] = a.w;
-    o.r[4] = c.x; o.r[5] = c.y; o.r[6] = c.z; o.r[7] = c.w;
-    return o;
-}
-RP_DEV void store_row_smem_at(int16_t* row, uint32_t p0, uint32_t p1, const Row8& v) {
-    U4* b = reinterpret_cast<U4*>(row);
-    b[p0] = U4{v.r[0], v.r[1], v.r[2], v.r[3]};
-    b[p1] = U4{v.r[4], v.r[5], v.r[6], v.r[7]};
 }
 RP_DEV void store_row_smem(int16_t* row, int lane, const Row8& v) {
     uint32_t q0 = 2u * static_cast<uint32_t>(lane);
@@ -360,6 +346,26 @@ struct PoaWarp {
     static RP_DEV uint32_t band_elem_smem(uint32_t c) {
         const uint32_t e = (((c >> 4) & (NB - 1)) << 4) | (perm_band(c) & 15u);
         return KB == 16 ? swz_e(e) : e;
+    }
+    /* Full-matrix rows in shared memory (the profile chunk and the DP ring): lane l's first granule (registers 0..3) at
+     * element 8l, its second (registers 4..7) at 8l + kCC/2.  Each LDS.128 / STS.128 of a row then covers 16 consecutive
+     * bytes per lane (bank-conflict free), and both take one address, the second at a constant offset. */
+    static RP_DEV uint32_t smem_elem(uint32_t c) {   // c = column inside the chunk
+        const uint32_t e = perm(c);
+        return ((e >> 3) & 1u) * (kCC / 2) + ((e >> 4) << 3) + (e & 7u);
+    }
+    static RP_DEV Row8 load_row_lane(const int16_t* at) {   // at = row + 8 * lane
+        const U4* b = reinterpret_cast<const U4*>(at);
+        const U4 a = b[0], c = b[G];
+        Row8 o;
+        o.r[0] = a.x; o.r[1] = a.y; o.r[2] = a.z; o.r[3] = a.w;
+        o.r[4] = c.x; o.r[5] = c.y; o.r[6] = c.z; o.r[7] = c.w;
+        return o;
+    }
+    static RP_DEV void store_row_lane(int16_t* at, const Row8& v) {
+        U4* b = reinterpret_cast<U4*>(at);
+        b[0] = U4{v.r[0], v.r[1], v.r[2], v.r[3]};
+        b[G] = U4{v.r[4], v.r[5], v.r[6], v.r[7]};
     }
     static RP_DEV void syncwarp() { gsync<G>(); }
     static RP_DEV uint32_t ballot(bool p) { return gballot<G>(p); }
@@ -707,7 +713,7 @@ struct PoaWarp {
                 uint32_t col = ch * kCC + cc;
                 int16_t v = static_cast<int16_t>(x);
                 if (col >= 1 && col <= len && seq[col - 1] == c) v = static_cast<int16_t>(m);
-                row[swz(cc)] = v;
+                row[smem_elem(cc)] = v;
             }
         }
     }
@@ -746,28 +752,29 @@ struct PoaWarp {
          * the carry between chunks goes through a small per-row array), so shared memory only ever holds one
          * chunk: the profile chunk and a ring of the last `ring_rows` rows. */
         const int32_t g = P->gap;
-        const uint32_t g2 = P->row_consts[16];
         const uint32_t nch = CHUNKS ? lpa / kCC : 1u;
-        const int32_t negsafe = -32768 - 16 * g;  // see kMaxGapInt16
-        const uint32_t* gb = P->row_consts;       // bridge / carry offsets per register (constant bank, see PoaParams)
+        /* The row loop's scalar constants, held in registers for the whole DP: taken by value from the parameter block,
+         * ptxas rather re-reads them from the constant bank at every use (and rebuilds 16g and negsafe from g in every
+         * row); a value that comes out of a shuffle it cannot re-read, so it keeps it. */
+        const uint32_t g2 = shfl(P->row_consts[16], 0);
+        const int32_t g16 = shfl(16 * g, 0);
+        const int32_t negsafe = shfl(-32768 - 16 * g, 0);  // see kMaxGapInt16
+        /* the per-register offsets stay operands from the constant bank (as registers they do not fit the kernel's
+         * register budget: ptxas spills) */
+        const uint32_t* gb = P->row_consts;       // bridge / carry offsets per register (see PoaParams)
         const uint32_t* gc = P->row_consts + 8;
         for (uint32_t col = lane; col < lpa; col += G) H[perm(col)] = static_cast<int16_t>(static_cast<int32_t>(col) * g);
-        const uint32_t sink_ch = len / kCC, sink_e = swz(len % kCC);
-        int32_t best = kNeg32;
-        uint32_t bi = 0, nb = 0;
         int16_t* cc_prev = ccarry;        // last column of the previous chunk, per row (multi-chunk rows only)
         int16_t* cc_cur = ccarry + (nmax + 2);
         const uint32_t lanem = static_cast<uint32_t>(lane);
-        /* this lane's two granules of a shared-memory row (load_row_smem's swizzle), pinned in registers for the row
-         * loop: re-derived per row they start every row's dependency chain with an S2R of the thread index */
-        uint32_t sw0 = (2u * lanem) ^ (((2u * lanem) >> 3) & 1u);
-        uint32_t sw1 = (2u * lanem + 1u) ^ (((2u * lanem + 1u) >> 3) & 1u);
-        RP_KEEP_IN_REGISTER(sw0);
-        RP_KEEP_IN_REGISTER(sw1);
+        /* this lane's place in a shared-memory row (smem_elem), pinned in a register for the row loop: re-derived per
+         * row it starts every row's dependency chain with an S2R of the thread index */
+        uint32_t lofs = 8u * lanem;
+        RP_KEEP_IN_REGISTER(lofs);
         for (uint32_t ch = 0; ch < nch; ++ch) {
             build_profile(seq, len, ch);
             for (uint32_t c = lane; c < kCC; c += G)  // root row (rank 0) -> ring slot 0
-                ring[swz(c)] = static_cast<int16_t>(static_cast<int32_t>(ch * kCC + c) * g);
+                ring[smem_elem(c)] = static_cast<int16_t>(static_cast<int32_t>(ch * kCC + c) * g);
             syncwarp();
             const bool multi = CHUNKS && ch > 0;
             /* columns beyond the read's last one are computed but never read by anything that matters (dependencies run
@@ -775,13 +782,15 @@ struct PoaWarp {
             const bool scan_lane = ch * kCC + lanem * 16u <= len;
             uint32_t rec_a_lo = 0, rec_a_hi = 0, rec_b_lo = 0, rec_b_hi = 0;
             int16_t* hrow = H + static_cast<uint64_t>(ch) * kCC;  // row i of this chunk = hrow + i*lpa
+            const int16_t* prof_l = keep_smem_ptr(prof + lofs);
+            int16_t* ring_l = keep_smem_ptr(ring + lofs);
             uint32_t myslot = 0;  // i % ring_rows, kept incrementally (any ring size, no division)
             /* where this lane stores its 16 columns of row i in the HBM copy: a running pointer (rows come in order), so
              * that the row loop carries one 64-bit add instead of rebuilding the address from the parameter block */
             U4* hst = reinterpret_cast<U4*>(hrow + lpa) + 2u * lanem;
-            Row8 prev;            // the row computed last (this lane's registers of it)
-#pragma unroll
-            for (int r = 0; r < 8; ++r) prev.r[r] = 0;
+            /* the row computed last (this lane's registers of it); the root row before row 1, whose only possible
+             * predecessor it is */
+            Row8 prev = load_row_lane(ring_l);
             /* rows in blocks of G: lane l fetches the record of row i0 + l once per block (a loop level of its own, so that
              * the row loop carries no predicated-off copy of the fetch), every row then takes its record by shuffle */
             Rec nxt = rec[1 + lane];  // rec[] is padded (SlotLayout: + 160 records)
@@ -798,14 +807,8 @@ struct PoaWarp {
               uint32_t lo_next = shfl(rec_a_lo, 0);
               for (uint32_t i = i0; i <= i_last; ++i) {
                 myslot = myslot + 1 == ring_rows ? 0u : myslot + 1;
-                const uint32_t ti = i - i0;
-                /* the record word of the NEXT row is shuffled out now: its latency runs under this row */
-                const uint32_t lo = lo_next;
-                lo_next = shfl(rec_a_lo, (ti + 1) & (G - 1));
-                const uint32_t cidx = lo & 0xff;
-                const uint32_t np = (lo >> 8) & 0x7f;
-                const bool sink = (lo >> 15) & 1;
-                const Row8 pf = load_row_smem_at(prof + cidx * kCC, sw0, sw1);
+                const uint32_t lo = lo_next;  // record word: code index | in-degree | sink | first predecessor
+                const Row8 pf = load_row_lane(prof_l + (lo & 0xff) * kCC);
                 /* max over predecessors distributes over both terms of the recurrence:
                  *   max_p(H[p][c-1] + s(c), H[p][c] + g) = max(max_p H[p][c-1] + s(c), max_p H[p][c] + g),
                  * so predecessor rows are first combined with a packed max (8 ops per extra predecessor) and the
@@ -816,7 +819,7 @@ struct PoaWarp {
                     const uint32_t dist = i - p;
                     if (__builtin_expect(dist < ring_rows, 1)) {  // warp-uniform; 98 % of the predecessors
                         const uint32_t slot = myslot >= dist ? myslot - dist : myslot + ring_rows - dist;
-                        pr = load_row_smem_at(ring + slot * kCC, sw0, sw1);
+                        pr = load_row_lane(ring_l + slot * kCC);
                     } else
                         pr = load_row_far(hrow + static_cast<uint64_t>(p) * lpa, lane);
                     if (multi) {
@@ -833,8 +836,8 @@ struct PoaWarp {
                 /* the first predecessor is loaded by every group of the warp together; only the groups whose row has
                  * more predecessors enter the nested part */
                 {
-                    const uint32_t p0 = np ? (lo >> 16) : 0u;
-                    if (p0 + 1 == i && p0 != 0) {  // group-uniform
+                    const uint32_t p0 = lo >> 16;  // 0 (the root row) when the row has no predecessor
+                    if (p0 + 1 == i) {  // group-uniform
                         /* the first predecessor is the row just computed (4 of 10 rows): it still is in registers — no
                          * trip through the shared-memory ring, whose store -> load latency would start this row */
                         pm = prev;
@@ -846,7 +849,9 @@ struct PoaWarp {
                         load_pred(p0, pm);
                     }
                 }
-                if (np > 1) {
+                if (lo & 0x7e00u) {  // in-degree > 1
+                    const uint32_t np = (lo >> 8) & 0x7f;
+                    const uint32_t ti = i - i0;
                     const uint32_t hi = shfl(rec_a_hi, ti);
                     more(hi & 0xffff);
                     if (np > 2) {
@@ -861,6 +866,9 @@ struct PoaWarp {
                         }
                     }
                 }
+                /* the record word of the next row, from lane (i + 1 - i0) mod G = i mod G (i0 = 1 mod G); shuffled here,
+                 * next to this row's own shuffle, its latency runs under the rest of the row */
+                lo_next = shfl(rec_a_lo, static_cast<int>(i & (G - 1)));
                 uint32_t acc[8];
                 {
                     uint32_t left = shfl_up(pm.r[7], 1);  // hi half = previous lane's last column
@@ -877,7 +885,7 @@ struct PoaWarp {
 #pragma unroll
                 for (int r = 1; r < 8; ++r) acc[r] = viaddmax_s16x2(acc[r - 1], g2, acc[r]);
                 /* bridge: column 7 feeds columns 8..15 */
-                const uint32_t bridge = byte_perm(acc[7], 0x80008000u, 0x1076);  // lo = INT16_MIN, hi = acc[7].lo
+                const uint32_t bridge = (acc[7] << 16) | 0x8000u;  // lo = INT16_MIN, hi = acc[7].lo
 #pragma unroll
                 for (int r = 0; r < 8; ++r) acc[r] = viaddmax_s16x2(bridge, gb[r], acc[r]);
                 /* warp max-plus scan of the lane totals (column 15 of each block), decay 16*g per lane */
@@ -891,12 +899,12 @@ struct PoaWarp {
                  * case; the scan stays for the rows where a long gap run really wins.) */
                 int32_t carry = shfl_up(t, 1);
                 carry = lanem == 0 ? chunk_carry : carry;
-                if (ballot(scan_lane && carry + 16 * g > t)) {  // group-uniform
-                    t = viaddmax_s32(lanem == 0 ? chunk_carry : kNeg32, 16 * g, t);
+                if (ballot(scan_lane && carry + g16 > t)) {  // group-uniform
+                    t = viaddmax_s32(lanem == 0 ? chunk_carry : kNeg32, g16, t);
 #pragma unroll
                     for (int dd = 1; dd < G; dd <<= 1) {
                         int32_t o = shfl_up(t, dd);
-                        t = viaddmax_s32(lanem >= static_cast<uint32_t>(dd) ? o : kNeg32, dd * 16 * g, t);
+                        t = viaddmax_s32(lanem >= static_cast<uint32_t>(dd) ? o : kNeg32, dd * g16, t);
                     }
                     carry = shfl_up(t, 1);
                     carry = lanem == 0 ? chunk_carry : carry;
@@ -909,23 +917,12 @@ struct PoaWarp {
 #pragma unroll
                 for (int r = 0; r < 8; ++r) out.r[r] = acc[r];
                 prev = out;
-                int16_t* myrow_s = ring + myslot * kCC;
-                store_row_smem_at(myrow_s, sw0, sw1, out);
+                /* each lane reads back only the ring granules it stored itself: no warp barrier between rows */
+                store_row_lane(ring_l + myslot * kCC, out);
                 hst[0] = U4{out.r[0], out.r[1], out.r[2], out.r[3]};
                 hst[1] = U4{out.r[4], out.r[5], out.r[6], out.r[7]};
                 hst += CHUNKS ? lpa / 8u : kCC / 8u;   // next row (a U4 holds 8 cells; one chunk: lpa == kCC)
                 if (CHUNKS && lanem == G - 1) cc_cur[i] = static_cast<int16_t>(hi16(acc[7]));
-                syncwarp();
-                if (sink && ch == sink_ch) {  // warp-uniform
-                    int32_t sc = myrow_s[sink_e];
-                    if (sc > best) {
-                        best = sc;
-                        bi = i;
-                        nb = 1;
-                    } else if (sc == best) {
-                        ++nb;
-                    }
-                }
               }
             }
             if (CHUNKS) {
@@ -936,9 +933,38 @@ struct PoaWarp {
                 syncwarp();
             }
         }
-        *best_row = bi;
-        *best_score = best;
-        *n_best = nb;
+        /* The sink rows' scores (column len) are read back from the HBM copy once the matrix is done, the rows spread over
+         * the lanes: a sink test in the row loop costs a divergent branch in every row, and sink rows are few.  Same
+         * result as the row order: the best score, the first row (lowest rank) that reaches it, and how many do. */
+        syncwarp();  // publishes the HBM copy: column len of a row was stored by the lane that owns it
+        int32_t best = kNeg32;
+        uint32_t bi = 0, nb = 0;
+        for (uint32_t r = 1 + lanem; r <= nrows; r += G) {
+            if (!((rec[r].a >> 15) & 1)) continue;
+            const int32_t sc = hcell<false>(lpa, r, len);
+            if (sc > best) {
+                best = sc;
+                bi = r;
+                nb = 1;
+            } else if (sc == best) {
+                ++nb;
+            }
+        }
+        for (int d = G / 2; d > 0; d >>= 1) {
+            const int32_t ob = shfl_down(best, d);
+            const uint32_t oi = shfl_down(bi, d), on = shfl_down(nb, d);
+            if (ob > best) {
+                best = ob;
+                bi = oi;
+                nb = on;
+            } else if (ob == best) {
+                bi = oi < bi ? oi : bi;
+                nb += on;
+            }
+        }
+        *best_row = shfl(bi, 0);
+        *best_score = shfl(best, 0);
+        *n_best = shfl(nb, 0);
         syncwarp();
     }
 

@@ -23,6 +23,7 @@
 #define RP_HD inline
 #define RP_GLOBAL
 #define RP_KEEP_IN_REGISTER(x) do { } while (0)
+template <typename T> inline T* keep_smem_ptr(T* p) { return p; }
 #else
 #include <cuda_runtime.h>
 #define RP_DEV __device__ __forceinline__
@@ -31,6 +32,13 @@
 /* makes a 32-bit value opaque to the compiler at this point: it then has to keep it in a register instead of
  * re-deriving it (from the thread index, the parameter block ...) inside a loop.  No instruction is emitted. */
 #define RP_KEEP_IN_REGISTER(x) asm volatile("" : "+r"(x))
+/* the same for a pointer into shared memory: its 32-bit shared-window address is pinned, so that an address derived from
+ * it inside a loop costs one add, and the accesses stay LDS/STS */
+template <typename T> __device__ __forceinline__ T* keep_smem_ptr(T* p) {
+    uint32_t a = static_cast<uint32_t>(__cvta_generic_to_shared(p));
+    RP_KEEP_IN_REGISTER(a);
+    return static_cast<T*>(__cvta_shared_to_generic(a));
+}
 #endif
 
 namespace rp {
