@@ -17,8 +17,8 @@
  *   * distance by k doubling, starting at the widest band that still fits one round (any k that succeeds gives
  *     the exact distance); Hirschberg columns with k = the known score of the sub-problem, the forward and the
  *     reverse pass of a node side by side in the two half-warps when the band fits 16 words; base cases store the
- *     vertical-(+1) and horizontal-(+1) bit-vectors of every band word and are walked back with edlib's move
- *     priority, the stored words of 32 columns at a time held in the lanes;
+ *     vertical-(+1) and horizontal-(+1) bit-vectors of every band word (two sibling leaves side by side, by the same
+ *     pass) and are walked back with edlib's move priority, the stored words of 32 columns at a time held in the lanes;
  *   * operations are written backwards into one buffer (right sub-problem first), run-length encoded, and — when
  *     a window length is set — turned into racon's breaking points (src/overlap.cpp:226-292) by the same warp.
  */
@@ -163,6 +163,21 @@ struct AlnWarp {
         syncwarp();
     }
 
+    /* One problem of a banded pass: the (n x m) matrix of the query whose match masks are peq against t (read
+     * backwards when rev_t), threshold k, columns 0..stop_col.  col receives the stop column (mode 1); spv, sph and
+     * sfirst are the store set a mode-2 pass fills. */
+    struct BandProblem {
+        const uint64_t* peq;
+        const uint8_t* t;
+        bool rev_t;
+        uint32_t n, m;
+        int32_t k;
+        uint32_t stop_col;
+        int32_t* col;
+        uint64_t *spv, *sph;
+        uint32_t* sfirst;
+    };
+
     /* One banded pass over columns 0..stop_col of the (n x m) problem with threshold k.
      * mode 0: returns H[n-1][stop_col] (the distance when stop_col == m-1), kAlnInf if the band misses it;
      * mode 1: additionally writes col[r+1] = H[r][stop_col] for every row r (kAlnInf outside the band),
@@ -170,10 +185,10 @@ struct AlnWarp {
      * mode 2: additionally stores the vertical-(+1) and horizontal-(+1) words of every column (base case). */
     RP_DEV int32_t band_pass(const uint64_t* peq, uint32_t n, const uint8_t* t, uint32_t m, bool rev_t, int32_t k,
                              uint32_t stop_col, int mode, int32_t* col) {
+        const BandProblem pr{peq, t, rev_t, n, m, k, stop_col, col, store_pv, store_ph, store_first};
         const int32_t span = band_span(n, m, k);
-        if (span <= 32) return band_pass_t<1, 32>(peq, peq, n, t, m, rev_t, rev_t, k, stop_col, stop_col, mode, col, col);
-        if (span <= 32 * kAlnSlots)
-            return band_pass_t<kAlnSlots, 32>(peq, peq, n, t, m, rev_t, rev_t, k, stop_col, stop_col, mode, col, col);
+        if (span <= 32) return band_pass_t<1, 32>(pr, pr, mode);
+        if (span <= 32 * kAlnSlots) return band_pass_t<kAlnSlots, 32>(pr, pr, mode);
         fail(kAlnBandLimit);
         return kAlnInf;
     }
@@ -193,7 +208,7 @@ struct AlnWarp {
     RP_DEV void band_pass_pair(const uint64_t* peq_a, const uint64_t* peq_b, uint32_t n, const uint8_t* t, uint32_t m,
                                int32_t k, uint32_t stop_a, uint32_t stop_b, int32_t* col_a, int32_t* col_b) {
         if (band_span(n, m, k) <= 16) {
-            band_pass_t<1, 16>(peq_a, peq_b, n, t, m, false, true, k, stop_a, stop_b, 1, col_a, col_b);
+            band_pass_t<1, 16>({peq_a, t, false, n, m, k, stop_a, col_a}, {peq_b, t, true, n, m, k, stop_b, col_b}, 1);
         } else {
             band_pass(peq_a, n, t, m, false, k, stop_a, 1, col_a);
             if (status != kAlnOk) return;
@@ -209,26 +224,30 @@ struct AlnWarp {
 
     /* SLOTS = band words a lane may hold at once.  With a band of <= W words (SLOTS = 1) the word that enters at
      * the bottom always lands in the lane whose previous word has just left at the top.
-     * W = lanes per problem: 32 (one problem, the *_a arguments) or 16 (problem a in lanes 0-15, b in lanes 16-31;
-     * same n, m, k; SLOTS = 1, mode 1 only). */
+     * W = lanes per problem: 32 (one problem, a; b is not read) or 16 (problem a in lanes 0-15, b in lanes 16-31,
+     * each with its own n, m, k, target and store set; SLOTS = 1, so every band fits one round of 16 words).
+     * Every lane returns its own problem's result. */
     template <int SLOTS, int W>
-    RP_DEV int32_t band_pass_t(const uint64_t* peq_a, const uint64_t* peq_b, uint32_t n, const uint8_t* t, uint32_t m,
-                               bool rev_a, bool rev_b, int32_t k, uint32_t stop_a, uint32_t stop_b, int mode,
-                               int32_t* col_a, int32_t* col_b) {
+    RP_DEV int32_t band_pass_t(const BandProblem& a, const BandProblem& b, int mode) {
         static_assert(W == 32 || (W == 16 && SLOTS == 1), "two problems per warp need single-slot bands");
-        const bool second = W == 16 && lane >= 16;
-        const uint64_t* peq = second ? peq_b : peq_a;
-        const bool rev_t = second ? rev_b : rev_a;
-        const uint32_t stop_col = second ? stop_b : stop_a;
-        int32_t* col = second ? col_b : col_a;
+        const bool second = W == 16 && lane >= 16;   // field by field: a selected reference would keep both in memory
+        const uint64_t* peq = second ? b.peq : a.peq;
+        const uint8_t* t = second ? b.t : a.t;
+        const bool rev_t = second ? b.rev_t : a.rev_t;
+        const uint32_t n = second ? b.n : a.n, m = second ? b.m : a.m, stop_col = second ? b.stop_col : a.stop_col;
+        const int32_t k = second ? b.k : a.k;
+        int32_t* col = second ? b.col : a.col;
+        uint64_t* spv = second ? b.spv : a.spv;
+        uint64_t* sph = second ? b.sph : a.sph;
+        uint32_t* sfirst = second ? b.sfirst : a.sfirst;
         const int sl = lane & (W - 1);        // my lane inside the problem's lane group
         const int gbase = lane & ~(W - 1);    // first lane of the group
-        const uint32_t last_col = stop_a > stop_b ? stop_a : stop_b;
+        const uint32_t last_col = W == 16 && b.stop_col > a.stop_col ? b.stop_col : a.stop_col;
 
         const int32_t delta = static_cast<int32_t>(n) - static_cast<int32_t>(m);
         const int32_t dlo = -((k - delta) / 2), dhi = (k + delta) / 2;  // diagonals i - j a cost-<=k path can touch
         const uint32_t nw = (n + 63) / 64;
-        if (dhi < 0 || dlo > 0) {  // k < |delta|: the band misses the corner cell (callers never ask for this)
+        if (ballot(dhi < 0 || dlo > 0)) {  // k < |delta|: a band misses its corner cell (callers never ask for this)
             fail(kAlnInternal);
             return kAlnInf;
         }
@@ -245,7 +264,7 @@ struct AlnWarp {
         uint32_t sidx_next = lut[rev_t ? t[m - 1] : t[0]];
         uint32_t tc_next = stop_col >= 1 ? (rev_t ? t[m - 2] : t[1]) : 0;
         for (uint32_t j = 0; j <= last_col; ++j) {
-            const bool live = j <= stop_col;   // the other half-warp's problem may run one column longer
+            const bool live = j <= stop_col;   // the other half-warp's problem may run longer
             int32_t rlo = static_cast<int32_t>(j) + dlo, rhi = static_cast<int32_t>(j) + dhi;
             if (rlo < 0) rlo = 0;
             if (rhi > n1) rhi = n1;
@@ -276,9 +295,12 @@ struct AlnWarp {
             const bool known = sidx < nsyms;
             int32_t carry = 1;  // horizontal delta entering the top word of the band (edlib.cpp:766: hout = 1)
             int32_t last_hout = 0;
-            if (mode == 2 && lane == 0) store_first[j] = (static_cast<uint32_t>(wlo) << 16) | static_cast<uint32_t>(whi - wlo + 1);
-            /* rounds of W consecutive words */
-            for (int32_t w0 = wlo; w0 <= whi; w0 += W) {
+            if (mode == 2 && live && sl == 0)
+                sfirst[j] = (static_cast<uint32_t>(wlo) << 16) | static_cast<uint32_t>(whi - wlo + 1);
+            /* rounds of W consecutive words; with two problems per warp exactly one in both halves, also in a half
+             * whose problem has ended (its band may then be empty) */
+            const int32_t wend = W == 16 ? wlo : whi;
+            for (int32_t w0 = wlo; w0 <= wend; w0 += W) {
                 const int rot = w0 & (W - 1);
                 const int pos = (sl - rot) & (W - 1);    // my word's position inside the round
                 const int32_t w = w0 + pos;              // the word of this round that lives in my lane
@@ -335,8 +357,8 @@ struct AlnWarp {
                     if (mode == 2) {
                         const uint64_t spos = store_pos + static_cast<uint64_t>(w - wlo);
                         if (spos < P->lim.store_words) {
-                            store_pv[spos] = Pvn;
-                            store_ph[spos] = Ph;
+                            spv[spos] = Pvn;
+                            sph[spos] = Ph;
                         } else {
                             status = kAlnStoreLimit;
                         }
@@ -347,14 +369,12 @@ struct AlnWarp {
                 last_hout = shfl(hout, gbase | (last_w & (W - 1)));
                 carry = last_hout;
             }
-            if (mode == 2) {
-                store_pos += static_cast<uint64_t>(whi - wlo + 1);
-                if (ballot(status != kAlnOk)) {  // some lane ran out of store space
-                    fail(kAlnStoreLimit);
-                    return kAlnInf;
-                }
+            if (mode == 2 && ballot(status != kAlnOk)) {  // some lane ran out of store space
+                fail(kAlnStoreLimit);
+                return kAlnInf;
             }
             if (live) {
+                if (mode == 2) store_pos += static_cast<uint64_t>(whi - wlo + 1);
                 sb += last_hout;
                 whi_prev = whi;
             }
@@ -363,14 +383,14 @@ struct AlnWarp {
         const int32_t j = static_cast<int32_t>(stop_col);
         int32_t rlo = j + dlo, rhi = j + dhi;
         if (rlo < 0) rlo = 0;
-        if (rhi > static_cast<int32_t>(n) - 1) rhi = static_cast<int32_t>(n) - 1;
+        if (rhi > n1) rhi = n1;
         const int32_t wlo = rlo >> 6, whi = rhi >> 6;
         int32_t result = kAlnInf;
         if (mode == 1)
             for (uint32_t r = sl; r <= n; r += W) col[r] = (r == 0) ? j + 1 : kAlnInf;
         syncwarp();
         /* walk the words from the bottom of the band up; words of one round are handled together.  With two problems
-         * per warp the band is a single round, so the loop bounds below are the same for every lane that matters. */
+         * per warp each band is a single round, so every lane runs the loop below once. */
         int32_t below = 0;  // sum of vertical deltas of all words below the current round
         const int32_t rounds = W == 16 ? 1 : (whi - wlo) / W + 1;
         for (int32_t rd = 0; rd < rounds; ++rd) {
@@ -408,29 +428,28 @@ struct AlnWarp {
                 if (mode == 1) {
                     for (int b = 63; b >= 0; --b) {
                         const int32_t r = w * 64 + b;
-                        if (r < static_cast<int32_t>(n) && r >= rlo && r <= rhi) {
-                            const uint64_t above = b == 63 ? 0ull : (~0ull << (b + 1));
-                            col[r + 1] = hbot - (popc64(Pv & above) - popc64(Mv & above));
-                        }
+                        if (r <= n1 && r >= rlo && r <= rhi) col[r + 1] = h_in_word(hbot, Pv, Mv, b);
                     }
                 }
-                const int32_t rl = static_cast<int32_t>(n) - 1;
-                if ((rl >> 6) == w && rl >= rlo && rl <= rhi) {
-                    const int b = rl & 63;
-                    const uint64_t above = b == 63 ? 0ull : (~0ull << (b + 1));
-                    result = hbot - (popc64(Pv & above) - popc64(Mv & above));
-                }
+                if ((n1 >> 6) == w && n1 >= rlo && n1 <= rhi) result = h_in_word(hbot, Pv, Mv, n1 & 63);
             }
             below += round_sum;
         }
-        /* the lane that owns row n-1 holds the result (W == 16: the first problem's) */
+        /* the lane that owns row n-1 holds the result: the minimum over each group ends in its first lane */
         for (int d = W / 2; d > 0; d >>= 1) {
             int32_t o = shfl_down(result, d);
             result = o < result ? o : result;
         }
-        result = shfl(result, 0);
+        result = shfl(result, gbase);
         syncwarp();
         return result;
+    }
+
+    /* H at row b of a band word whose bottom row (b = 63) holds hbot: hbot minus the vertical deltas of the rows
+     * below b (the Pv / Mv bits above bit b) */
+    RP_DEV static int32_t h_in_word(int32_t hbot, uint64_t Pv, uint64_t Mv, int b) {
+        const uint64_t above = b == 63 ? 0ull : (~0ull << (b + 1));
+        return hbot - (popc64(Pv & above) - popc64(Mv & above));
     }
 
     RP_DEV void fail(uint32_t st) {
@@ -545,124 +564,24 @@ struct AlnWarp {
     }
 
 
-    /* Two sibling leaves of the Hirschberg tree side by side, one per half-warp (their bands are a few words wide):
-     * leaf A (left child: peq_f, store set 1) in lanes 0-15, leaf B (right child: peq_r, store set 2) in lanes 16-31;
-     * each with its own n, m, k.  Same recurrence as band_pass_t in mode 2, single round, W = 16. */
+    /* Two sibling leaves of the Hirschberg tree whose bands fit 16 words, filled side by side by one two-problem
+     * pass: leaf A (left child: peq_f, store set 1) in lanes 0-15, leaf B (right child: peq_r, store set 2) in lanes
+     * 16-31.  Then both are walked, the right leaf first: operations are written backwards. */
     RP_DEV void leaf_pair(const uint8_t* qa, uint32_t na, const uint8_t* ta, uint32_t ma, int32_t ka, const uint8_t* qb,
                           uint32_t nb, const uint8_t* tb, uint32_t mb, int32_t kb, uint32_t* wpos) {
-        constexpr int W = 16;
 #if defined(RP_HOST_SIM)
         if (lane == 0) ++g_sim_leaf_pairs;
 #endif
         build_peq(peq_f, qa, na, false);
         build_peq(peq_r, qb, nb, false);
-        const bool second = lane >= 16;
-        const uint64_t* peq = second ? peq_r : peq_f;
-        const uint8_t* t = second ? tb : ta;
-        const uint32_t n = second ? nb : na, m = second ? mb : ma;
-        const int32_t k = second ? kb : ka;
-        uint64_t* spv = second ? store2_pv : store_pv;
-        uint64_t* sph = second ? store2_ph : store_ph;
-        uint32_t* sfirst = second ? store2_first : store_first;
-        const int sl = lane & (W - 1), gbase = lane & ~(W - 1);
-        const int32_t delta = static_cast<int32_t>(n) - static_cast<int32_t>(m);
-        const int32_t dlo = -((k - delta) / 2), dhi = (k + delta) / 2;
-        const uint32_t nw = (n + 63) / 64;
-        const int32_t n1 = static_cast<int32_t>(n) - 1;
-        if (ballot(dhi < 0 || dlo > 0)) {
+        const int32_t d =
+            band_pass_t<1, 16>({peq_f, ta, false, na, ma, ka, ma - 1, nullptr, store_pv, store_ph, store_first},
+                               {peq_r, tb, false, nb, mb, kb, mb - 1, nullptr, store2_pv, store2_ph, store2_first}, 2);
+        if (status != kAlnOk) return;
+        if (ballot(d != (lane < 16 ? ka : kb))) {  // each leaf must reproduce its known score
             fail(kAlnInternal);
             return;
         }
-        uint64_t Pv = ~0ull, Mv = 0;
-        int32_t whi_prev = -1, sb = 0;
-        uint64_t store_pos = 0;
-        uint32_t sidx_next = lut[t[0]];
-        uint32_t tc_next = m > 1 ? t[1] : 0;
-        const uint32_t cols = ma > mb ? ma : mb;
-        int32_t whi = 0;
-        for (uint32_t j = 0; j < cols; ++j) {
-            const bool live = j < m;
-            int32_t rlo = static_cast<int32_t>(j) + dlo, rhi = static_cast<int32_t>(j) + dhi;
-            if (rlo < 0) rlo = 0;
-            if (rhi > n1) rhi = n1;
-            const int32_t wlo = rlo >> 6;
-            if (live) whi = rhi >> 6;
-            if (live) {
-                if (j == 0) {
-                    sb = 64 * (whi + 1);
-                } else if (whi != whi_prev) {
-                    sb += 64;
-                    if ((whi & (W - 1)) == sl) {
-                        Pv = ~0ull;
-                        Mv = 0;
-                    }
-                }
-            }
-            const uint32_t sidx = sidx_next;
-            sidx_next = lut[tc_next];
-            if (j + 2 < m) tc_next = t[j + 2];
-            const bool known = sidx < nsyms;
-            const uint64_t* peq_row = peq + static_cast<uint64_t>(known ? sidx : 0) * nw;
-            const int rot = wlo & (W - 1);
-            const int pos = (sl - rot) & (W - 1);
-            const int32_t w = wlo + pos;
-            const bool act = live && w <= whi;
-            const uint64_t Eq = (act && known) ? peq_row[w] : 0ull;
-            const uint64_t Eq1 = Eq | 1ull;
-            const uint64_t Xh0 = (((Eq & Pv) + Pv) ^ Pv) | Eq;
-            const uint64_t Xh1 = (((Eq1 & Pv) + Pv) ^ Pv) | Eq1;
-            const bool neg0 = act && ((Pv & Xh0) >> 63) != 0;
-            const bool neg1 = act && ((Pv & Xh1) >> 63) != 0;
-            const uint32_t gen = rotr_w(ballot(neg0) >> gbase, rot, W);
-            const uint32_t prop = rotr_w(ballot(neg1 && !neg0) >> gbase, rot, W);
-            const uint32_t negin = ((gen | prop) + gen) ^ prop;  // carry into the top word is +1: never negative
-            const bool hneg = ((negin >> pos) & 1u) != 0;
-            const uint64_t Xh = hneg ? Xh1 : Xh0;
-            const uint64_t Xv = Eq | Mv;
-            const uint64_t Ph = Mv | ~(Xh | Pv);
-            const uint64_t Mh = Pv & Xh;
-            const int32_t hout = act ? static_cast<int32_t>(Ph >> 63) - static_cast<int32_t>(Mh >> 63) : 0;
-            int32_t hin = shfl(hout, gbase | ((sl + W - 1) & (W - 1)));
-            if (pos == 0) hin = 1;
-            const uint64_t Phs = (Ph << 1) | (hin > 0 ? 1ull : 0ull);
-            const uint64_t Mhs = (Mh << 1) | (hneg ? 1ull : 0ull);
-            if (act) {
-                Pv = Mhs | ~(Xv | Phs);
-                Mv = Phs & Xv;
-                const uint64_t spos = store_pos + static_cast<uint64_t>(w - wlo);
-                if (spos < P->lim.store_words) {
-                    spv[spos] = Pv;
-                    sph[spos] = Ph;
-                } else {
-                    status = kAlnStoreLimit;
-                }
-            }
-            const int32_t last_hout = shfl(hout, gbase | (whi & (W - 1)));
-            if (live) {
-                if (sl == 0) sfirst[j] = (static_cast<uint32_t>(wlo) << 16) | static_cast<uint32_t>(whi - wlo + 1);
-                store_pos += static_cast<uint64_t>(whi - wlo + 1);
-                sb += last_hout;
-                whi_prev = whi;
-            }
-        }
-        if (ballot(status != kAlnOk)) {
-            fail(kAlnStoreLimit);
-            return;
-        }
-        /* each leaf must reproduce its known score: H[n-1][m-1] = bottom score minus the vertical deltas below row n-1 */
-        int32_t d = 0;
-        if (sl == ((n1 >> 6) & (W - 1))) {
-            const int bb = n1 & 63;
-            const uint64_t above = bb == 63 ? 0ull : (~0ull << (bb + 1));
-            d = sb - (popc64(Pv & above) - popc64(Mv & above));
-        }
-        d = shfl(d, gbase | ((n1 >> 6) & (W - 1)));
-        if (ballot(d != k)) {
-            fail(kAlnInternal);
-            return;
-        }
-        syncwarp();
-        /* operations are written backwards: the right leaf first */
         walk_stored(nb, mb, store2_pv, store2_ph, store2_first, col_r, wpos);
         if (status != kAlnOk) return;
         walk_stored(na, ma, store_pv, store_ph, store_first, col_l, wpos);
@@ -745,6 +664,12 @@ struct AlnWarp {
         return overflow ? 0xffffffffu : nb;
     }
 
+    /* edlib's 1 MiB rule (edlib.cpp:1155-1157): an (n x m) problem whose bit-vectors take less than 1 MiB is a base
+     * case, traced back from its stored band; a larger one is split */
+    RP_DEV static bool below_1mib_rule(uint32_t n, uint32_t m) {
+        return 20ull * ((n + 63) / 64) * m + 8ull * m < 1024ull * 1024ull;
+    }
+
     /* whole pair: distance, Hirschberg recursion (explicit stack), run-length encoding */
     RP_DEV void align_pair(uint32_t p) {
         const uint8_t* q = P->bases + P->q_off[p];
@@ -808,7 +733,7 @@ struct AlnWarp {
                 const int32_t kmax = static_cast<int32_t>(n > m ? n : m);
                 /* a pair below edlib's 1 MiB rule is traced back from stored bit-vectors: store them right here
                  * (any band that contains the optimal paths serves), so the pair needs no second pass */
-                direct = 20ull * ((n + 63) / 64) * m + 8ull * m < 1024ull * 1024ull;
+                direct = below_1mib_rule(n, m);
                 for (;;) {
                     int32_t diff = static_cast<int32_t>(n) - static_cast<int32_t>(m);
                     if (diff < 0) diff = -diff;
@@ -854,9 +779,7 @@ struct AlnWarp {
                     emit_run(ql == 0 ? 'D' : 'I', ql + tl, &wpos);
                     continue;
                 }
-                const uint64_t blocks = (ql + 63) / 64;
-                const uint64_t data = 20ull * blocks * tl + 8ull * tl;  // edlib.cpp:1155-1157
-                if (data < 1024ull * 1024ull) {
+                if (below_1mib_rule(ql, tl)) {
                     base_case(q + qo, ql, t + to, tl, b, &wpos, direct && ql == n && tl == m);
                     continue;
                 }
@@ -901,11 +824,8 @@ struct AlnWarp {
                     break;
                 }
                 const uint32_t qa_n = ul, qb_n = ql - ul;
-                auto is_leaf = [](uint32_t qn, uint32_t tn) {
-                    return 20ull * ((qn + 63) / 64) * tn + 8ull * tn < 1024ull * 1024ull;  // edlib.cpp:1155-1157
-                };
-                if (qa_n > 0 && qb_n > 0 && lw > 0 && rw > 0 && is_leaf(qa_n, lw) && is_leaf(qb_n, rw) &&
-                    band_span(qa_n, lw, ls) <= 16 && band_span(qb_n, rw, rs) <= 16) {
+                if (qa_n > 0 && qb_n > 0 && lw > 0 && rw > 0 && below_1mib_rule(qa_n, lw) &&
+                    below_1mib_rule(qb_n, rw) && band_span(qa_n, lw, ls) <= 16 && band_span(qb_n, rw, rs) <= 16) {
                     /* both children are base cases with narrow bands: fill them side by side, then walk right, left */
                     leaf_pair(q + qo, qa_n, t + to, lw, ls, q + qo + ul, qb_n, t + to + lw, rw, rs, &wpos);
                     continue;
