@@ -1398,8 +1398,16 @@ struct PoaWarp {
         return 0;
     }
 
+    /* true when the band that starts at block s really cuts the matrix (an edge at column 0 or at the last block cuts
+     * nothing) closer than `margin` columns to col_l on the left or to col_r on the right (see traceback) */
+    static RP_DEV bool near_cut_edge(uint32_t s, uint32_t col_l, uint32_t col_r, uint32_t nblk, uint32_t margin) {
+        const int32_t dl = static_cast<int32_t>(col_l) - static_cast<int32_t>(16u * s);
+        const int32_t dr = static_cast<int32_t>(16u * (s + NB)) - 1 - static_cast<int32_t>(col_r);
+        return (s > 0 && dl < static_cast<int32_t>(margin)) || (s + NB < nblk && dr < static_cast<int32_t>(margin));
+    }
+
     /* banded walk, more predecessors than lanes: true when some candidate cell is closer than the margin to an edge
-     * that cuts its own row's band (see traceback) */
+     * that cuts its own row's band */
     static RP_DEV_NOINLINE bool wide_candidates_unsure(const uint8_t* bs, const Rec* rec, const uint16_t* pred_ovf,
                                                        uint32_t ki, int lane, uint32_t i, uint32_t j, uint32_t npe,
                                                        uint32_t nblk, uint32_t margin) {
@@ -1408,13 +1416,7 @@ struct PoaWarp {
             const uint32_t k = k0 + lane;
             if (k < npe) {
                 const uint32_t p = k < 7 ? rec_pred(rec[i], k) : pred_ovf[i * ki + k];
-                if (p != 0) {
-                    const uint32_t sp = bs[p];
-                    const int32_t dlp = static_cast<int32_t>(j) - 1 - static_cast<int32_t>(16u * sp);
-                    const int32_t drp = static_cast<int32_t>(16u * (sp + NB)) - 1 - static_cast<int32_t>(j);
-                    unsure |= (sp > 0 && dlp < static_cast<int32_t>(margin)) ||
-                              (sp + NB < nblk && drp < static_cast<int32_t>(margin));
-                }
+                if (p != 0) unsure |= near_cut_edge(bs[p], j - 1, j, nblk, margin);
             }
         }
         return gballot<G>(unsure) != 0;
@@ -1545,9 +1547,7 @@ struct PoaWarp {
             const uint32_t ejm = j > 0 ? pjm - t_col0 : 0;  // column j-1
             const int32_t hij = tile[q * kTileCols + ej];
             if (BAND) {
-                const uint32_t si = tbs[q];
-                const uint32_t dl = j - 16u * si, dr = 16u * (si + NB) - 1u - j;
-                if ((si > 0 && dl < margin) || (si + NB < nblk && dr < margin) || hij < worst) {  // group-uniform
+                if (near_cut_edge(tbs[q], j, j, nblk, margin) || hij < worst) {  // group-uniform
                     bad = true;
                     break;
                 }
@@ -1586,12 +1586,8 @@ struct PoaWarp {
                         b = hcell<BAND>(lpa, p, j);
                         sp = bs[p];
                     }
-                    if (BAND && p != 0) {  // the candidate cells must be trustworthy too (see the general case)
-                        const int32_t dlp = static_cast<int32_t>(j) - 1 - static_cast<int32_t>(16u * sp);
-                        const int32_t drp = static_cast<int32_t>(16u * (sp + NB)) - 1 - static_cast<int32_t>(j);
-                        unsure |= (sp > 0 && dlp < static_cast<int32_t>(margin)) ||
-                                  (sp + NB < nblk && drp < static_cast<int32_t>(margin));
-                    }
+                    // the candidate cells must be trustworthy too (see the general case)
+                    if (BAND && p != 0) unsure |= near_cut_edge(sp, j - 1, j, nblk, margin);
                     if (!okv && hij == b + g) {
                         okv = true;
                         pv = p;
@@ -1633,15 +1629,10 @@ struct PoaWarp {
                     }
                     okd = j > 0 && hij == a + mc;
                     okv = hij == b + g;
-                    if (BAND && p != 0) {
-                        /* the candidate cells (p, j-1), (p, j) must be trustworthy too: a predecessor whose own band is
-                         * cut closer than the margin to these columns (or does not hold them at all) could hide a tie
-                         * the full matrix would have resolved the other way */
-                        const int32_t dlp = static_cast<int32_t>(j) - 1 - static_cast<int32_t>(16u * sp);
-                        const int32_t drp = static_cast<int32_t>(16u * (sp + NB)) - 1 - static_cast<int32_t>(j);
-                        unsure = (sp > 0 && dlp < static_cast<int32_t>(margin)) ||
-                                 (sp + NB < nblk && drp < static_cast<int32_t>(margin));
-                    }
+                    /* the candidate cells (p, j-1), (p, j) must be trustworthy too: a predecessor whose own band is cut
+                     * closer than the margin to these columns (or does not hold them at all) could hide a tie the full
+                     * matrix would have resolved the other way */
+                    if (BAND && p != 0) unsure = near_cut_edge(sp, j - 1, j, nblk, margin);
                 }
                 if (BAND && ballot(unsure)) {  // group-uniform
                     bad = true;
@@ -2181,10 +2172,6 @@ RP_DEV int64_t worst_case_score(int32_t m, int32_t g, int64_t len, int64_t nodes
     int64_t b = g * i + g * j;
     return a < b ? a : b;
 }
-RP_DEV bool fits_int16(int32_t m, int32_t g, int64_t len, int64_t nodes) {
-    if (g < -kMaxGapInt16) return false;
-    return worst_case_score(m, g, len, nodes) >= static_cast<int64_t>(-32768 + 1024);
-}
 
 /* Processes one window end to end. `slot`: this group's HBM scratch, `smem`: this group's shared memory. */
 template <int G, int KB = 16>
@@ -2236,7 +2223,7 @@ RP_DEV void poa_window(const PoaParams& P, uint32_t w, uint8_t* slot, uint8_t* s
             if (W.status != kWinOk) break;
             nrows = W.build_dp_order_subgraph();
         }
-        /* spoa picks its int32 engine from a worst-case bound over ALL nodes of the graph (fits_int16).  That bound
+        /* spoa picks its int32 engine from a worst-case bound over ALL nodes of the graph (`fits`).  That bound
          * is far from what a real matrix holds (column 0 only falls by |g| per level of graph DEPTH), and exact
          * arithmetic gives the same answer in either width, so a window that fails the bound is still computed in
          * int16 and the finished matrix is checked for having stayed in range (matrix_in_range).  The bound says
