@@ -28,6 +28,7 @@ typedef int32_t rp_status;
 enum {
     RP_OK = 0,
     RP_BATCH_FULL = 1,      /* item not added: run the batch, reset, add it again (cudabatch.cpp:126-132) */
+    RP_NOT_READY = 2,       /* rp_poa_query / rp_aln_query: the last run is still in flight */
     RP_ERR_INVALID = -1,    /* bad argument / malformed window (the reference exit(1)s: window.cpp:19-23,49-58) */
     RP_ERR_CUDA = -2,       /* CUDA runtime failure; rp_last_error() has the text */
     RP_ERR_NOMEM = -3,
@@ -91,7 +92,8 @@ rp_status rp_poa_add_window(rp_poa* p, uint32_t n_seq, const char* const* seq, c
  *
  * rp_reads_create: data[i] / length[i] = sequence i (targets and reads, any order); quality[i] NULL (or quality NULL) =
  * no qualities.  The host arrays must stay valid while the store is alive (backbone copies of windows with < 3 sequences
- * and the rare exact alphabet scan read them).  One store can serve any number of batch objects on the same device. */
+ * and the rare exact alphabet scan read them).  One store can serve any number of batch objects on the same device, on
+ * any of their streams: nothing writes to a store after rp_reads_create has returned (its upload is complete by then). */
 typedef struct rp_reads rp_reads;
 rp_status rp_reads_create(rp_reads** out, int device, uint32_t n_seqs, const char* const* data,
                           const char* const* quality, const uint32_t* length);
@@ -129,6 +131,10 @@ uint32_t rp_poa_size(const rp_poa* p);    /* windows in the batch (CUDABatchProc
  * rp_poa_run = upload + launch + download, asynchronous on the object's stream; rp_poa_sync waits. */
 rp_status rp_poa_run(rp_poa* p);
 rp_status rp_poa_sync(rp_poa* p);
+/* Non-blocking completion test of the last run: RP_OK when it has finished (rp_poa_sync then returns without waiting
+ * for the device, unless windows have to be escalated), RP_NOT_READY while it is in flight, RP_ERR_STATE when nothing
+ * was launched since the last reset.  Lets one host thread keep batch objects on several devices busy. */
+rp_status rp_poa_query(rp_poa* p);
 /* the three stages separately (bench.py times rp_poa_launch alone with inputs resident in HBM) */
 rp_status rp_poa_upload(rp_poa* p);
 rp_status rp_poa_launch(rp_poa* p);
@@ -212,6 +218,8 @@ uint32_t rp_aln_size(const rp_aln* a);
 /* CUDABatchAligner::alignAll (async) / generate_cigar_strings (sync), cudaaligner.cpp:80-104 */
 rp_status rp_aln_run(rp_aln* a);
 rp_status rp_aln_sync(rp_aln* a);
+/* rp_poa_query for the aligner: RP_OK (finished), RP_NOT_READY (in flight) or RP_ERR_STATE (nothing launched) */
+rp_status rp_aln_query(rp_aln* a);
 rp_status rp_aln_upload(rp_aln* a);
 rp_status rp_aln_launch(rp_aln* a);
 rp_status rp_aln_download(rp_aln* a);

@@ -14,6 +14,7 @@ _lib = None
 
 RP_OK = 0
 RP_BATCH_FULL = 1
+RP_NOT_READY = 2
 
 
 class RaconB200Error(RuntimeError):
@@ -41,6 +42,7 @@ SIGNATURES = {
     "rp_poa_size": (_u32, [_vp]),
     "rp_poa_run": (_st, [_vp]),
     "rp_poa_sync": (_st, [_vp]),
+    "rp_poa_query": (_st, [_vp]),
     "rp_poa_upload": (_st, [_vp]),
     "rp_poa_launch": (_st, [_vp]),
     "rp_poa_download": (_st, [_vp]),
@@ -62,6 +64,7 @@ SIGNATURES = {
     "rp_aln_size": (_u32, [_vp]),
     "rp_aln_run": (_st, [_vp]),
     "rp_aln_sync": (_st, [_vp]),
+    "rp_aln_query": (_st, [_vp]),
     "rp_aln_upload": (_st, [_vp]),
     "rp_aln_launch": (_st, [_vp]),
     "rp_aln_download": (_st, [_vp]),
@@ -76,11 +79,11 @@ HOST_SIGNATURES = {
     "rp_mirror_align": (_int, [_u32, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _u32]),
     "rp_mirror_consensus": (C.c_double, [_u32] + [_vp] * 8 + [_i8, _i8, _i8, _u32, _int, _u32, _vp, _u32, _vp, _vp]),
     "rp_mirror_polisher_open": (_vp, [_u32, _vp, _vp, _vp, _vp, _u32, _int, _int, _u32, _vp, _u32, C.c_double, _int,
-                                      _i8, _i8, _i8, _u32]),
+                                      _i8, _i8, _i8, _vp, _u32]),
     "rp_mirror_polisher_open_with_bp": (_vp, [_u32, _vp, _vp, _vp, _vp, _u32, _int, _int, _u32, _vp, _vp, _vp, _u32,
                                               C.c_double]),
     "rp_mirror_polisher_open_files": (_vp, [_str, _str, _str, _int, _u32, C.c_double, C.c_double, _int, _i8, _i8, _i8,
-                                            _u32, _int, _vp, _u32]),
+                                            _vp, _u32, _int, _vp, _u32]),
     "rp_mirror_polisher_counts": (None, [_vp, _vp]),
     "rp_mirror_polisher_export": (None, [_vp] * 11),
     "rp_mirror_polisher_polish": (_u32, [_vp, _int]),
@@ -88,8 +91,10 @@ HOST_SIGNATURES = {
     "rp_mirror_polisher_polished": (_u64, [_vp, _u32, _vp, _vp, _u32, _vp, _u64]),
     "rp_mirror_polisher_close": (None, [_vp]),
     "rp_mirror_polisher_failed": (None, [_vp, _vp]),
+    "rp_mirror_polisher_breaking_points": (_u64, [_vp, _vp, _vp]),
     "rp_mirror_polisher_stream_fasta": (_u32, [_vp, _int, _str, _str, _u64, _int, _int]),
     "rp_mirror_format_fasta": (_u64, [_str, _str, _str, _u64, _str, _u64]),
+    "rp_mirror_stitch_order": (_u64, [_u32, _vp, _vp, _vp, _vp]),
     "rp_mirror_input_open": (_vp, [_str, _str, _str, _int, C.c_double, _vp, _u32]),
     "rp_mirror_input_counts": (None, [_vp, _vp]),
     "rp_mirror_input_export": (None, [_vp] * 8),
@@ -141,6 +146,28 @@ def _check(lib, st, what):
 
 def _ptr(a):
     return None if a is None else a.ctypes.data
+
+
+def device_count():
+    """CUDA devices the library sees (rp_device_count; 0 without one): device=range(device_count()) uses them all."""
+    return max(0, int(load().rp_device_count()))
+
+
+def _device_list(device):
+    """device: one CUDA device index or a sequence of them, one lane each (an index may repeat: [0, 0] = two lanes on
+    GPU 0) -> the uint32 array the host layer takes.  Raises RaconB200Error on an empty list or an index that no visible
+    device has; without any device nothing can be checked here and the first device call fails instead ("no CUDA
+    device", as for a single index)."""
+    devices = [device] if isinstance(device, (int, np.integer)) else list(device)
+    if not devices:
+        raise RaconB200Error("empty device list")
+    n = device_count()
+    for d in devices:
+        if isinstance(d, bool) or not isinstance(d, (int, np.integer)):
+            raise RaconB200Error("device index %r is not an integer" % (d,))
+        if d < 0 or (n > 0 and d >= n):
+            raise RaconB200Error("device index %d out of range: %d CUDA device(s) visible" % (d, n))
+    return np.ascontiguousarray(devices, dtype=np.uint32)
 
 
 class ReadStore:
@@ -292,6 +319,10 @@ class PoaBatch:
     def sync(self):
         _check(self.lib, self.lib.rp_poa_sync(self.h), "rp_poa_sync")
 
+    def ready(self):
+        """True when the last run has finished, False while it is in flight (rp_poa_query; never blocks)."""
+        return _check(self.lib, self.lib.rp_poa_query(self.h), "rp_poa_query") == RP_OK
+
     def reset(self):
         _check(self.lib, self.lib.rp_poa_reset(self.h), "rp_poa_reset")
 
@@ -404,6 +435,10 @@ class AlnBatch:
     def sync(self):
         _check(self.lib, self.lib.rp_aln_sync(self.h), "rp_aln_sync")
 
+    def ready(self):
+        """True when the last run has finished, False while it is in flight (rp_aln_query; never blocks)."""
+        return _check(self.lib, self.lib.rp_aln_query(self.h), "rp_aln_query") == RP_OK
+
     def reset(self):
         _check(self.lib, self.lib.rp_aln_reset(self.h), "rp_aln_reset")
 
@@ -480,8 +515,9 @@ class MirrorPolisher:
     def __init__(self, bases, quals, seq_off, seq_has_qual, n_targets, overlaps, window_length=500,
                  quality_threshold=10.0, trim=True, match=3, mismatch=-5, gap=-4, window_type_tgs=True,
                  fragment_correction=False, device=0, breaking_points=None):
-        """breaking_points=(bp_off, bp): skip the device alignment and build the windows from given breaking points
-        (host logic only; no GPU needed, polish() is then not available)."""
+        """device: a CUDA device index or a sequence of them (one lane each, see host_mirror.hpp's Polisher; an index may
+        repeat).  breaking_points=(bp_off, bp): skip the device alignment and build the windows from given breaking
+        points (host logic only; no GPU needed, `device` is not used and polish() is then not available)."""
         self.lib = load()
         L = self.lib
         # keep the sequence bytes alive: the windows point into them
@@ -490,6 +526,7 @@ class MirrorPolisher:
         self._off = np.ascontiguousarray(seq_off, dtype=np.uint64)
         self._hq = np.ascontiguousarray(seq_has_qual, dtype=np.uint8)
         ov = np.ascontiguousarray(overlaps, dtype=np.uint32)
+        self._n_overlaps = len(ov)
         if breaking_points is not None:
             bp_off = np.ascontiguousarray(breaking_points[0], dtype=np.uint64)
             bp = np.ascontiguousarray(breaking_points[1], dtype=np.uint32)
@@ -499,24 +536,30 @@ class MirrorPolisher:
                                                        len(ov), _ptr(ov), _ptr(bp_off), _ptr(bp), window_length,
                                                        quality_threshold)
             return
+        devices = _device_list(device)
         self.h = L.rp_mirror_polisher_open(len(self._off) - 1, _ptr(self._bases), _ptr(self._quals), _ptr(self._off),
                                            _ptr(self._hq), n_targets, 1 if window_type_tgs else 0,
                                            1 if fragment_correction else 0, len(ov), _ptr(ov), window_length,
-                                           quality_threshold, 1 if trim else 0, match, mismatch, gap, device)
+                                           quality_threshold, 1 if trim else 0, match, mismatch, gap, _ptr(devices),
+                                           len(devices))
 
     @classmethod
     def from_files(cls, reads, overlaps, targets, fragment_correction=False, window_length=500, quality_threshold=10.0,
                    error_threshold=0.3, trim=True, match=3, mismatch=-5, gap=-4, device=0, resident_reads=False):
         """createPolisher + initialize on files (reads_io.hpp): parse, filter, align + breaking points on the device
-        (SAM input keeps its own alignments and needs no device here), build the windows.  resident_reads: the sequences
-        are uploaded once and the aligner (and later the consensus) name their inputs instead of copying them."""
+        (SAM input keeps its own alignments and needs no device here), build the windows.  device: a CUDA device index
+        or a sequence of them, one lane each (an index may repeat); both device stages spread their batches over the
+        lanes.  resident_reads: the sequences are uploaded once per device and the aligner (and later the consensus) name
+        their inputs instead of copying them."""
         self = cls.__new__(cls)
         self.lib = load()
+        self._n_overlaps = None
+        devices = _device_list(device)
         err = C.create_string_buffer(1024)
         self.h = self.lib.rp_mirror_polisher_open_files(os.fsencode(reads), os.fsencode(overlaps), os.fsencode(targets),
                                                         1 if fragment_correction else 0, window_length, quality_threshold,
-                                                        error_threshold, 1 if trim else 0, match, mismatch, gap, device,
-                                                        1 if resident_reads else 0, err, 1024)
+                                                        error_threshold, 1 if trim else 0, match, mismatch, gap,
+                                                        _ptr(devices), len(devices), 1 if resident_reads else 0, err, 1024)
         if not self.h:
             raise RuntimeError(err.value.decode(errors="replace"))
         return self
@@ -553,13 +596,25 @@ class MirrorPolisher:
         return cons, out
 
     def stream_fasta(self, path, names, drop_unpolished=False, mem_bytes=0, banded=False, resident_reads=False):
-        """Polisher::polish_streaming into a FASTA file: two batch objects in flight, every polished sequence written the
-        moment its last window is collected (polisher.cpp:504-537 + main.cpp:159-161).  names: target names by id
-        (None: the names of the files a from_files() polisher was opened on).  resident_reads: every sequence is
-        uploaded once and the windows are added by reference (layers extracted on the device)."""
+        """Polisher::polish_streaming into a FASTA file: two batch objects in flight per device lane, every polished
+        sequence written in target order the moment its last window is stitched (polisher.cpp:504-537 +
+        main.cpp:159-161).  names: target names by id (None: the names of the files a from_files() polisher was opened
+        on).  resident_reads: every sequence is uploaded once per device and the windows are added by reference (layers
+        extracted on the device)."""
         blob = None if names is None else b"".join(n.encode() + b"\0" for n in names) + b"\0"
         return self.lib.rp_mirror_polisher_stream_fasta(self.h, 1 if drop_unpolished else 0, os.fsencode(path), blob,
                                                         mem_bytes, 1 if banded else 0, 1 if resident_reads else 0)
+
+    def breaking_points(self):
+        """(bp_off, bp) of a polisher opened on arrays: the (t, q) breaking points of overlap i are
+        bp[bp_off[i]:bp_off[i + 1]] — what the aligner stage produced (empty for an overlap the device refused)."""
+        if self._n_overlaps is None:
+            raise RaconB200Error("breaking_points: only for a polisher opened on arrays")
+        n = int(self.lib.rp_mirror_polisher_breaking_points(self.h, None, None))
+        off = np.zeros(self._n_overlaps + 1, np.uint64)
+        bp = np.zeros((max(n, 1), 2), np.uint32)
+        self.lib.rp_mirror_polisher_breaking_points(self.h, _ptr(off), _ptr(bp))
+        return off, bp[:n]
 
     def failed(self):
         """(overlaps, windows) the device could not finish (see host_mirror.hpp: Polisher::failed_overlaps/windows)."""
@@ -612,6 +667,20 @@ def consensus(ws, match=3, mismatch=-5, gap=-4, trim=True, window_length=500, de
     if want_coverage:
         return cons, pol, st, covs
     return cons, pol, st
+
+
+def stitch_order(counts, completion):
+    """The polisher's stitch cursor (host logic only): contiguous ranges of counts[r] windows finish in the order
+    `completion`.  Returns (windows in the order they were stitched, for each the index into `completion` of the finish
+    that stitched it)."""
+    lib = load()
+    counts = np.ascontiguousarray(counts, dtype=np.uint32)
+    completion = np.ascontiguousarray(completion, dtype=np.uint32)
+    total = int(counts.sum())
+    order = np.zeros(max(total, 1), np.uint64)
+    step = np.zeros(max(total, 1), np.uint32)
+    n = lib.rp_mirror_stitch_order(len(counts), _ptr(counts), _ptr(completion), _ptr(order), _ptr(step))
+    return order[:n], step[:n]
 
 
 def mirror_consensus(ws, match=3, mismatch=-5, gap=-4, trim=True, window_length=500, device=0):
@@ -684,7 +753,9 @@ def polish_files(reads, overlaps, targets, out_path, fragment_correction=False, 
                  error_threshold=0.3, trim=True, match=3, mismatch=-5, gap=-4, device=0, drop_unpolished=True,
                  mem_bytes=0, banded=False, resident_reads=True):
     """racon's whole run through the C++ host layer: files in, polished FASTA out (alignment, breaking points and
-    consensus on the device).  Returns (records written, overlaps the device refused, windows the device refused)."""
+    consensus on the device).  device: a CUDA device index or a sequence of them — device=range(device_count()) runs on
+    every visible GPU; the file is byte-identical whatever the list.  Returns (records written, overlaps the device
+    refused, windows the device refused)."""
     pol = MirrorPolisher.from_files(reads, overlaps, targets, fragment_correction=fragment_correction,
                                     window_length=window_length, quality_threshold=quality_threshold,
                                     error_threshold=error_threshold, trim=trim, match=match, mismatch=mismatch, gap=gap,

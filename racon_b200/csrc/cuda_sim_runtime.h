@@ -17,7 +17,7 @@
 #include <cstring>
 
 typedef int cudaError_t;
-enum { cudaSuccess = 0, cudaErrorMemoryAllocation = 2, cudaErrorNoDevice = 100 };
+enum { cudaSuccess = 0, cudaErrorMemoryAllocation = 2, cudaErrorNoDevice = 100, cudaErrorNotReady = 600 };
 typedef struct rp_sim_stream* cudaStream_t;
 enum { cudaStreamNonBlocking = 1, cudaHostAllocDefault = 0 };
 enum cudaMemcpyKind { cudaMemcpyHostToDevice = 1, cudaMemcpyDeviceToHost = 2, cudaMemcpyDeviceToDevice = 3 };
@@ -107,6 +107,7 @@ inline cudaError_t cudaStreamDestroy(cudaStream_t s) {
     return cudaSuccess;
 }
 inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
+inline cudaError_t cudaStreamQuery(cudaStream_t) { return cudaSuccess; }   // the work of a stream is done when queued
 template <typename F>
 inline cudaError_t cudaFuncSetAttribute(F, int, int) {
     return cudaSuccess;

@@ -7,12 +7,34 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <iterator>
+#include <stdexcept>
 
 #include "racon_b200.h"
 #include "reads_io.hpp"
 
 namespace racon_b200 {
+namespace {
+
+/* A hard error (negative rp_status) ends the process with a message, as the reference's batch objects do.  A device stage
+ * of the polisher owns several batch objects and read stores: while it runs (run_stage) the error is thrown instead, the
+ * stage's objects are destroyed on the way out, and the read stores are released before the same message is printed. */
+thread_local int hard_error_scopes = 0;
+
+struct HardError : std::runtime_error {
+    using std::runtime_error::runtime_error;
+};
+
+[[noreturn]] void hard_error(const std::string& message) {
+    if (hard_error_scopes > 0) throw HardError(message);
+    fprintf(stderr, "%s\n", message.c_str());
+    exit(1);
+}
+
+std::string status_text(rp_status s) { return std::string(rp_strerror(s)) + " (" + rp_last_error() + ")"; }
+
+}  // namespace
 
 std::shared_ptr<Window> createWindow(uint64_t id, uint32_t rank, WindowType type, const char* backbone,
                                      uint32_t backbone_length, const char* quality, uint32_t quality_length) {
@@ -73,8 +95,7 @@ BatchProcessor::BatchProcessor(uint32_t max_window_depth, uint32_t device, size_
     rp_status s = rp_poa_create(&poa_, static_cast<int>(device), avail_mem, match, mismatch, gap,
                                 cuda_banded_alignment ? 1 : 0, window_length, max_window_depth);
     if (s != RP_OK) {  // hard failure, like GW_CU_CHECK_ERR / std::runtime_error in the reference
-        fprintf(stderr, "[racon_b200::BatchProcessor] error: %s (%s)\n", rp_strerror(s), rp_last_error());
-        exit(1);
+        hard_error("[racon_b200::BatchProcessor] error: " + status_text(s));
     }
 }
 
@@ -110,8 +131,7 @@ bool BatchProcessor::addWindow(std::shared_ptr<Window> window) {
     }
     if (s == RP_BATCH_FULL) return false;
     if (s != RP_OK) {
-        fprintf(stderr, "[racon_b200::BatchProcessor::addWindow] error: %s (%s)\n", rp_strerror(s), rp_last_error());
-        exit(1);
+        hard_error("[racon_b200::BatchProcessor::addWindow] error: " + status_text(s));
     }
     windows_.push_back(window);
     return true;
@@ -127,16 +147,14 @@ const std::vector<bool>& BatchProcessor::generateConsensus() {
 void BatchProcessor::launch() {
     const rp_status s = rp_poa_run(poa_);
     if (s != RP_OK) {
-        fprintf(stderr, "[racon_b200::BatchProcessor::launch] error: %s (%s)\n", rp_strerror(s), rp_last_error());
-        exit(1);
+        hard_error("[racon_b200::BatchProcessor::launch] error: " + status_text(s));
     }
 }
 
 const std::vector<bool>& BatchProcessor::collect() {
     const rp_status s = rp_poa_sync(poa_);
     if (s != RP_OK) {
-        fprintf(stderr, "[racon_b200::BatchProcessor::collect] error: %s (%s)\n", rp_strerror(s), rp_last_error());
-        exit(1);
+        hard_error("[racon_b200::BatchProcessor::collect] error: " + status_text(s));
     }
     window_consensus_status_.clear();
     failed_.clear();
@@ -163,6 +181,15 @@ const std::vector<bool>& BatchProcessor::collect() {
     return window_consensus_status_;
 }
 
+bool BatchProcessor::ready() {
+    const rp_status s = rp_poa_query(poa_);
+    if (s == RP_NOT_READY) return false;
+    if (s != RP_OK) {
+        hard_error("[racon_b200::BatchProcessor::ready] error: " + status_text(s));
+    }
+    return true;
+}
+
 void BatchProcessor::reset() {
     windows_.clear();
     window_consensus_status_.clear();
@@ -184,8 +211,7 @@ BatchAligner::BatchAligner(uint32_t max_query_size, uint32_t max_target_size, ui
     rp_status s = rp_aln_create(&aln_, static_cast<int>(device_id), 0,
                                 max_query_size > max_target_size ? max_query_size : max_target_size);
     if (s != RP_OK) {
-        fprintf(stderr, "[racon_b200::BatchAligner] error: %s (%s)\n", rp_strerror(s), rp_last_error());
-        exit(1);
+        hard_error("[racon_b200::BatchAligner] error: " + status_text(s));
     }
 }
 
@@ -196,8 +222,7 @@ bool BatchAligner::addOverlap(const char* q, uint32_t q_len, const char* t, uint
     rp_status s = rp_aln_add(aln_, q, q_len, t, t_len);
     if (s == RP_BATCH_FULL) return false;
     if (s != RP_OK) {
-        fprintf(stderr, "[racon_b200::BatchAligner::addOverlap] error: %s (%s)\n", rp_strerror(s), rp_last_error());
-        exit(1);
+        hard_error("[racon_b200::BatchAligner::addOverlap] error: " + status_text(s));
     }
     cigars_.push_back(cigar);
     return true;
@@ -206,17 +231,14 @@ bool BatchAligner::addOverlap(const char* q, uint32_t q_len, const char* t, uint
 void BatchAligner::alignAll() {
     rp_status s = rp_aln_run(aln_);
     if (s != RP_OK) {
-        fprintf(stderr, "[racon_b200::BatchAligner::alignAll] error: %s (%s)\n", rp_strerror(s), rp_last_error());
-        exit(1);
+        hard_error("[racon_b200::BatchAligner::alignAll] error: " + status_text(s));
     }
 }
 
 void BatchAligner::generate_cigar_strings() {
     rp_status s = rp_aln_sync(aln_);
     if (s != RP_OK) {
-        fprintf(stderr, "[racon_b200::BatchAligner::generate_cigar_strings] error: %s (%s)\n", rp_strerror(s),
-                rp_last_error());
-        exit(1);
+        hard_error("[racon_b200::BatchAligner::generate_cigar_strings] error: " + status_text(s));
     }
     for (uint32_t i = 0; i < cigars_.size(); ++i) {
         const char* c = nullptr;
@@ -244,39 +266,102 @@ std::string format_fasta(const std::string& target_name, const PolishedSequence&
 }
 
 /* ---- Polisher ---- */
+namespace {
+
+/* The scheduler of both device stages.  Lane l is idle or busy; fill(l) hands an idle lane the next piece of work and
+ * launches it (false: nothing left), ready(l) tests a busy lane without blocking, drain(l) collects a finished one.  Every
+ * idle lane is refilled before the next collect; the lane collected is one that has finished, else the oldest in flight
+ * (waiting on it instead of polling in a loop). */
+template <typename Fill, typename Ready, typename Drain>
+void run_lanes(size_t n_lanes, Fill&& fill, Ready&& ready, Drain&& drain) {
+    std::vector<uint8_t> busy(n_lanes, 0);
+    std::deque<size_t> in_flight;   // busy lanes, oldest launch first
+    while (true) {
+        for (size_t l = 0; l < n_lanes; ++l) {
+            if (!busy[l] && fill(l)) {
+                busy[l] = 1;
+                in_flight.push_back(l);
+            }
+        }
+        if (in_flight.empty()) return;
+        auto it = std::find_if(in_flight.begin(), in_flight.end(), [&](size_t l) { return ready(l); });
+        if (it == in_flight.end()) it = in_flight.begin();
+        const size_t l = *it;
+        in_flight.erase(it);
+        busy[l] = 0;
+        drain(l);
+    }
+}
+
+/* Runs one device stage of the polisher: on a hard error anywhere inside, the stage's batch objects (its locals) are
+ * destroyed while the error leaves it, then release() frees the read stores, then the process ends with the message. */
+template <typename Stage, typename Release>
+void run_stage(Stage&& stage, Release&& release) {
+    ++hard_error_scopes;
+    try {
+        stage();
+    } catch (const HardError& e) {
+        --hard_error_scopes;
+        release();
+        fprintf(stderr, "%s\n", e.what());
+        exit(1);
+    }
+    --hard_error_scopes;
+}
+
+}  // namespace
+
 Polisher::Polisher(std::vector<SequenceView> sequences, uint64_t targets_size, WindowType window_type,
                    bool fragment_correction, uint32_t window_length, double quality_threshold, bool trim, int8_t match,
-                   int8_t mismatch, int8_t gap, uint32_t device)
+                   int8_t mismatch, int8_t gap, std::vector<uint32_t> devices)
     : sequences_(std::move(sequences)), targets_size_(targets_size), window_type_(window_type),
       fragment_correction_(fragment_correction), window_length_(window_length), quality_threshold_(quality_threshold),
-      trim_(trim), match_(match), mismatch_(mismatch), gap_(gap), device_(device),
+      trim_(trim), match_(match), mismatch_(mismatch), gap_(gap), devices_(std::move(devices)),
       dummy_quality_(window_length, '!'),  // polisher.cpp:174
       reverse_complement_(sequences_.size()), reverse_quality_(sequences_.size()) {
     if (window_length == 0) {  // polisher.cpp:71-75
         fprintf(stderr, "[racon_b200::Polisher] error: invalid window length!\n");
         exit(1);
     }
-}
-
-Polisher::~Polisher() { rp_reads_destroy(store_); }
-
-const rp_reads* Polisher::read_store() {
-    if (store_ == nullptr) {
-        std::vector<const char*> data(sequences_.size()), quality(sequences_.size());
-        std::vector<uint32_t> length(sequences_.size());
-        for (size_t i = 0; i < sequences_.size(); ++i) {
-            data[i] = sequences_[i].data;
-            quality[i] = sequences_[i].quality;
-            length[i] = sequences_[i].length;
-        }
-        const rp_status s = rp_reads_create(&store_, static_cast<int>(device_), static_cast<uint32_t>(data.size()),
-                                            data.data(), quality.data(), length.data());
-        if (s != RP_OK) {
-            fprintf(stderr, "[racon_b200::Polisher] error: read store: %s (%s)\n", rp_strerror(s), rp_last_error());
+    if (devices_.empty()) {
+        fprintf(stderr, "[racon_b200::Polisher] error: empty device list!\n");
+        exit(1);
+    }
+    /* without any device no index can be checked: the first device call then fails with "no CUDA device", as for one
+     * index (SAM input builds its windows without a device) */
+    const int count = rp_device_count();
+    for (uint32_t d : devices_) {
+        if (count > 0 && d >= static_cast<uint32_t>(count)) {
+            fprintf(stderr, "[racon_b200::Polisher] error: device %u out of range (%d CUDA devices)!\n", d, count);
             exit(1);
         }
     }
-    return store_;
+}
+
+Polisher::~Polisher() { release_read_stores(); }
+
+void Polisher::release_read_stores() {
+    for (auto& s : stores_) rp_reads_destroy(s.second);
+    stores_.clear();
+}
+
+/* rp_reads is read-only once rp_reads_create has returned, so every batch object on `device` shares its one store */
+const rp_reads* Polisher::read_store(uint32_t device) {
+    for (const auto& s : stores_)
+        if (s.first == device) return s.second;
+    std::vector<const char*> data(sequences_.size()), quality(sequences_.size());
+    std::vector<uint32_t> length(sequences_.size());
+    for (size_t i = 0; i < sequences_.size(); ++i) {
+        data[i] = sequences_[i].data;
+        quality[i] = sequences_[i].quality;
+        length[i] = sequences_[i].length;
+    }
+    rp_reads* store = nullptr;
+    const rp_status s = rp_reads_create(&store, static_cast<int>(device), static_cast<uint32_t>(data.size()),
+                                        data.data(), quality.data(), length.data());
+    if (s != RP_OK) hard_error("[racon_b200::Polisher] error: read store: " + status_text(s));
+    stores_.emplace_back(device, store);
+    return store;
 }
 
 const char* Polisher::reverse_complement(uint32_t id) {  // Sequence::create_reverse_complement, sequence.cpp:58-93
@@ -325,52 +410,72 @@ void Polisher::find_overlap_breaking_points(std::vector<Overlap>& overlaps) {
         }
     }
     if (todo.empty()) return;
-    rp_aln* aln = nullptr;
-    rp_status s = rp_aln_create(&aln, static_cast<int>(device_), 0, longest);
-    if (s == RP_OK) s = rp_aln_set_window_length(aln, window_length_);
-    if (s != RP_OK) {
-        fprintf(stderr, "[racon_b200::Polisher::find_overlap_breaking_points] error: %s (%s)\n", rp_strerror(s),
-                rp_last_error());
-        exit(1);
+    run_stage([&] { align(overlaps, todo, longest); }, [&] { release_read_stores(); });
+    std::sort(failed_overlaps_.begin(), failed_overlaps_.end());   // lanes finish in any order
+}
+
+void Polisher::align(std::vector<Overlap>& overlaps, const std::vector<size_t>& todo, uint32_t longest) {
+    struct Lane {
+        std::unique_ptr<rp_aln, void (*)(rp_aln*)> aln{nullptr, rp_aln_destroy};
+        uint32_t device = 0;
+        size_t first = 0, end = 0;   // the lane's batch: todo[first, end)
+    };
+    std::vector<Lane> lanes(devices_.size());
+    /* a hard error on any lane ends the run like a single-device one (run_stage) */
+    auto fail = [](const std::string& what) {
+        hard_error("[racon_b200::Polisher::find_overlap_breaking_points] error: " + what);
+    };
+    for (size_t l = 0; l < lanes.size(); ++l) {
+        lanes[l].device = devices_[l];
+        rp_aln* aln = nullptr;
+        rp_status s = rp_aln_create(&aln, static_cast<int>(devices_[l]), 0, longest);
+        lanes[l].aln.reset(aln);
+        if (s == RP_OK) s = rp_aln_set_window_length(aln, window_length_);
+        if (s != RP_OK) fail(status_text(s));
     }
-    size_t i = 0;
-    while (i < todo.size()) {
-        const size_t first = i;
-        for (; i < todo.size(); ++i) {
-            const Overlap& o = overlaps[todo[i]];
+    size_t next = 0;   // the shared cursor over todo
+    auto fill = [&](size_t l) {
+        Lane& lane = lanes[l];
+        if (next == todo.size()) return false;
+        rp_aln* aln = lane.aln.get();
+        lane.first = next;
+        for (; next < todo.size(); ++next) {
+            const Overlap& o = overlaps[todo[next]];
             /* the spans racon hands to the aligner (overlap.cpp:193-197) */
             const uint32_t q_start = o.strand ? o.q_length - o.q_end : o.q_begin;
+            rp_status s;
             if (resident_reads_) {
-                s = rp_aln_add_overlap_ref(aln, read_store(), o.q_id, q_start, o.q_end - o.q_begin, o.strand != 0, o.t_id,
-                                           o.t_begin, o.t_end - o.t_begin);
+                s = rp_aln_add_overlap_ref(aln, read_store(lane.device), o.q_id, q_start, o.q_end - o.q_begin,
+                                           o.strand != 0, o.t_id, o.t_begin, o.t_end - o.t_begin);
             } else {
                 const char* q = (o.strand ? reverse_complement(o.q_id) : sequences_[o.q_id].data) + q_start;
                 const char* t = sequences_[o.t_id].data + o.t_begin;
                 s = rp_aln_add_overlap(aln, q, o.q_end - o.q_begin, t, o.t_end - o.t_begin, o.t_begin, q_start);
             }
             if (s == RP_BATCH_FULL) break;
-            if (s != RP_OK) {
-                fprintf(stderr, "[racon_b200::Polisher::find_overlap_breaking_points] error: %s (%s)\n",
-                        rp_strerror(s), rp_last_error());
-                exit(1);
-            }
+            if (s != RP_OK) fail(status_text(s));
         }
-        if (i == first) {
-            fprintf(stderr, "[racon_b200::Polisher::find_overlap_breaking_points] error: overlap does not fit an empty batch\n");
-            exit(1);
-        }
-        s = rp_aln_run(aln);
-        if (s == RP_OK) s = rp_aln_sync(aln);
-        if (s != RP_OK) {
-            fprintf(stderr, "[racon_b200::Polisher::find_overlap_breaking_points] error: %s (%s)\n", rp_strerror(s),
-                    rp_last_error());
-            exit(1);
-        }
-        for (size_t j = first; j < i; ++j) {
+        if (next == lane.first) fail("overlap does not fit an empty batch");
+        lane.end = next;
+        const rp_status s = rp_aln_run(aln);   // asynchronous: the host goes on filling the other lanes
+        if (s != RP_OK) fail(status_text(s));
+        return true;
+    };
+    auto ready = [&](size_t l) {
+        const rp_status s = rp_aln_query(lanes[l].aln.get());
+        if (s != RP_OK && s != RP_NOT_READY) fail(status_text(s));
+        return s == RP_OK;
+    };
+    auto drain = [&](size_t l) {
+        Lane& lane = lanes[l];
+        rp_aln* aln = lane.aln.get();
+        rp_status s = rp_aln_sync(aln);
+        if (s != RP_OK) fail(status_text(s));
+        for (size_t j = lane.first; j < lane.end; ++j) {
             const size_t k = todo[j];
             const uint32_t* pts = nullptr;
             uint32_t n = 0, st = 0;
-            rp_aln_fetch_cigar(aln, static_cast<uint32_t>(j - first), nullptr, nullptr, nullptr, &st);
+            rp_aln_fetch_cigar(aln, static_cast<uint32_t>(j - lane.first), nullptr, nullptr, nullptr, &st);
             if (st != RP_ALN_OK) {
                 /* the reference re-aligns such overlaps with its CPU edlib (cudapolisher.cpp:213); this path has no CPU
                  * aligner, so the overlap contributes no layers and the caller is told */
@@ -378,13 +483,14 @@ void Polisher::find_overlap_breaking_points(std::vector<Overlap>& overlaps) {
                 failed_overlaps_.push_back(k);
                 continue;
             }
-            rp_aln_fetch_breaking_points(aln, static_cast<uint32_t>(j - first), &pts, &n);
+            rp_aln_fetch_breaking_points(aln, static_cast<uint32_t>(j - lane.first), &pts, &n);
             overlaps[k].breaking_points_.clear();
             for (uint32_t b = 0; b < n; ++b) overlaps[k].breaking_points_.emplace_back(pts[2 * b], pts[2 * b + 1]);
         }
-        rp_aln_reset(aln);
-    }
-    rp_aln_destroy(aln);
+        s = rp_aln_reset(aln);
+        if (s != RP_OK) fail(status_text(s));
+    };
+    run_lanes(lanes.size(), fill, ready, drain);
 }
 
 void Polisher::initialize(std::vector<Overlap>& overlaps) {
@@ -445,63 +551,44 @@ void Polisher::build_windows(const std::vector<Overlap>& overlaps) {
 }
 
 void Polisher::polish(std::vector<PolishedSequence>& dst, bool drop_unpolished_sequences) {
-    auto batch = createBatch(0, device_, 0, gap_, mismatch_, match_, false, window_length_, trim_);
-    std::vector<bool> polished(windows_.size(), false);
-    size_t i = 0;
-    while (i < windows_.size()) {  // cudapolisher.cpp:254-276: fill, run, collect, reset
-        const size_t first = i;
-        while (i < windows_.size() && batch->addWindow(windows_[i])) ++i;
-        if (i == first) {
-            fprintf(stderr, "[racon_b200::Polisher::polish] error: window does not fit an empty batch\n");
-            exit(1);
-        }
-        const std::vector<bool>& flags = batch->generateConsensus();
-        for (size_t k = 0; k < flags.size(); ++k) polished[first + k] = flags[k];
-        for (uint32_t k : batch->failedWindows()) failed_windows_.push_back(first + k);
-        batch->reset();
-    }
-
-    /* stitch (polisher.cpp:504-537) */
-    std::string polished_data;
-    uint32_t num_polished_windows = 0;
-    for (uint64_t w = 0; w < windows_.size(); ++w) {
-        num_polished_windows += polished[w] ? 1 : 0;
-        polished_data += windows_[w]->consensus();
-        if (w == windows_.size() - 1 || windows_[w + 1]->rank() == 0) {
-            const double polished_ratio = num_polished_windows / static_cast<double>(windows_[w]->rank() + 1);
-            if (!drop_unpolished_sequences || polished_ratio > 0) {
-                std::string tags = fragment_correction_ ? "r" : "";
-                tags += " LN:i:" + std::to_string(polished_data.size());
-                tags += " RC:i:" + std::to_string(targets_coverages_[windows_[w]->id()]);
-                tags += " XC:f:" + std::to_string(polished_ratio);
-                dst.push_back(PolishedSequence{windows_[w]->id(), tags, polished_data});
-            }
-            num_polished_windows = 0;
-            polished_data.clear();
-        }
-    }
+    /* the windows are kept: their consensus stays readable (Polisher::windows) */
+    consensus([&](const PolishedSequence& p) { dst.push_back(p); }, drop_unpolished_sequences, 0, false,
+              resident_reads_, false);
 }
 
 void Polisher::polish_streaming(const std::function<void(const PolishedSequence&)>& sink,
                                 bool drop_unpolished_sequences, size_t memory, bool banded, bool resident_reads) {
-    constexpr int kObjects = 2;
-    struct InFlight {
+    consensus(sink, drop_unpolished_sequences, memory, banded, resident_reads || resident_reads_, true);
+}
+
+void Polisher::consensus(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
+                         size_t memory, bool banded, bool resident_reads, bool release) {
+    run_stage([&] { consensus_lanes(sink, drop_unpolished_sequences, memory, banded, resident_reads, release); },
+              [&] { release_read_stores(); });
+    std::sort(failed_windows_.begin(), failed_windows_.end());   // batches finish in any order
+}
+
+void Polisher::consensus_lanes(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
+                               size_t memory, bool banded, bool resident_reads, bool release) {
+    constexpr size_t kObjectsPerLane = 2;   // one runs on the device while the host fills / collects the other
+    struct Slot {
         std::unique_ptr<BatchProcessor> batch;
-        size_t first = 0, count = 0;
-        bool busy = false;
+        size_t first = 0, count = 0;   // the object's batch: windows [first, first + count)
     };
-    /* resident reads: every sequence goes to the device once; the windows (whose pieces know their origin, build_windows)
-     * are then added by reference and their layers extracted on the device */
-    const rp_reads* store = (resident_reads || resident_reads_) ? read_store() : nullptr;
-    InFlight obj[kObjects];
-    for (auto& o : obj) {
-        o.batch = createBatch(0, device_, memory, gap_, mismatch_, match_, banded, window_length_, trim_);
-        o.batch->useReadStore(store);
+    /* slot s runs on devices_[s % lanes]: the first round of batches goes to every lane before any gets a second */
+    std::vector<Slot> slots(kObjectsPerLane * devices_.size());
+    for (size_t i = 0; i < slots.size(); ++i) {
+        const uint32_t device = devices_[i % devices_.size()];
+        slots[i].batch = createBatch(0, device, memory, gap_, mismatch_, match_, banded, window_length_, trim_);
+        /* resident reads: every sequence goes to the device once; the windows (whose pieces know their origin,
+         * build_windows) are then added by reference and their layers extracted on the device */
+        slots[i].batch->useReadStore(resident_reads ? read_store(device) : nullptr);
     }
+    std::vector<uint8_t> polished(windows_.size(), 0);   // Window::generate_consensus' flag, until stitched
     std::string polished_data;
     uint32_t num_polished_windows = 0;
-    auto stitch = [&](size_t w, bool polished) {  // polisher.cpp:504-530, one window at a time, in window order
-        num_polished_windows += polished ? 1 : 0;
+    auto stitch = [&](size_t w) {  // polisher.cpp:504-530, one window at a time, in window order
+        num_polished_windows += polished[w];
         polished_data += windows_[w]->consensus();
         if (w == windows_.size() - 1 || windows_[w + 1]->rank() == 0) {
             const double polished_ratio = num_polished_windows / static_cast<double>(windows_[w]->rank() + 1);
@@ -515,35 +602,33 @@ void Polisher::polish_streaming(const std::function<void(const PolishedSequence&
             num_polished_windows = 0;
             polished_data.clear();
         }
-        windows_[w].reset();  // polisher.cpp:531: the window is not needed any more
+        if (release) windows_[w].reset();  // polisher.cpp:531: the window is not needed any more
     };
-    size_t next = 0;
-    int fill = 0, drain = 0;  // objects are filled and drained in the same round-robin order => window order
-    while (next < windows_.size() || obj[drain].busy) {
-        InFlight& f = obj[fill];
-        if (!f.busy && next < windows_.size()) {
-            f.batch->reset();
-            f.first = next;
-            while (next < windows_.size() && f.batch->addWindow(windows_[next])) ++next;
-            f.count = next - f.first;
-            if (f.count == 0) {
-                fprintf(stderr, "[racon_b200::Polisher::polish_streaming] error: window does not fit an empty batch\n");
-                exit(1);
-            }
-            f.batch->launch();  // asynchronous: the host goes on filling the other object / stitching
-            f.busy = true;
-            fill = (fill + 1) % kObjects;
-            if (!obj[fill].busy && next < windows_.size()) continue;  // keep both in flight before draining
+    InOrderStitcher stitcher(windows_.size());
+    size_t next = 0;   // the shared cursor over windows_
+    auto fill = [&](size_t i) {
+        Slot& slot = slots[i];
+        if (next == windows_.size()) return false;
+        slot.first = next;
+        while (next < windows_.size() && slot.batch->addWindow(windows_[next])) ++next;
+        slot.count = next - slot.first;
+        if (slot.count == 0) {
+            hard_error(std::string("[racon_b200::Polisher::") + (release ? "polish_streaming" : "polish") +
+                       "] error: window does not fit an empty batch");
         }
-        InFlight& d = obj[drain];
-        if (d.busy) {
-            const std::vector<bool>& flags = d.batch->collect();
-            for (uint32_t k : d.batch->failedWindows()) failed_windows_.push_back(d.first + k);
-            for (size_t k = 0; k < d.count; ++k) stitch(d.first + k, flags[k]);
-            d.busy = false;
-            drain = (drain + 1) % kObjects;
-        }
-    }
+        slot.batch->launch();  // asynchronous: the host goes on filling the other objects / stitching
+        return true;
+    };
+    auto ready = [&](size_t i) { return slots[i].batch->ready(); };
+    auto drain = [&](size_t i) {
+        Slot& slot = slots[i];
+        const std::vector<bool>& flags = slot.batch->collect();
+        for (uint32_t k : slot.batch->failedWindows()) failed_windows_.push_back(slot.first + k);
+        for (size_t k = 0; k < slot.count; ++k) polished[slot.first + k] = flags[k] ? 1 : 0;
+        slot.batch->reset();   // drops the batch's references to its windows
+        stitcher.finish(slot.first, slot.count, stitch);
+    };
+    run_lanes(slots.size(), fill, ready, drain);
 }
 
 }  // namespace racon_b200
@@ -555,6 +640,8 @@ struct PolHandle {
     std::unique_ptr<racon_b200::InputSet> input;   // owns the sequence bytes when the polisher was opened on files
     std::unique_ptr<racon_b200::Polisher> polisher;
     std::vector<racon_b200::PolishedSequence> polished;
+    std::vector<racon_b200::Overlap> overlaps;     // with their breaking points, when opened on arrays
+    const std::vector<racon_b200::Overlap>& all_overlaps() const { return input ? input->overlaps : overlaps; }
 };
 }  // namespace
 
@@ -562,7 +649,7 @@ extern "C" void* rp_mirror_polisher_open(uint32_t n_seq, const char* bases, cons
                                          const uint8_t* seq_has_qual, uint32_t n_targets, int window_type_tgs,
                                          int fragment_correction, uint32_t n_overlaps, const uint32_t* overlaps,
                                          uint32_t window_length, double quality_threshold, int trim, int8_t match,
-                                         int8_t mismatch, int8_t gap, uint32_t device) {
+                                         int8_t mismatch, int8_t gap, const uint32_t* devices, uint32_t n_devices) {
     using namespace racon_b200;
     std::vector<SequenceView> seqs(n_seq);
     for (uint32_t i = 0; i < n_seq; ++i) {
@@ -578,8 +665,9 @@ extern "C" void* rp_mirror_polisher_open(uint32_t n_seq, const char* bases, cons
     PolHandle* h = new PolHandle();
     h->polisher.reset(new Polisher(std::move(seqs), n_targets, window_type_tgs ? WindowType::kTGS : WindowType::kNGS,
                                    fragment_correction != 0, window_length, quality_threshold, trim != 0, match,
-                                   mismatch, gap, device));
+                                   mismatch, gap, std::vector<uint32_t>(devices, devices + n_devices)));
     h->polisher->initialize(ovl);
+    h->overlaps = std::move(ovl);
     return h;
 }
 
@@ -604,8 +692,9 @@ extern "C" void* rp_mirror_polisher_open_with_bp(uint32_t n_seq, const char* bas
     }
     PolHandle* h = new PolHandle();
     h->polisher.reset(new Polisher(std::move(seqs), n_targets, window_type_tgs ? WindowType::kTGS : WindowType::kNGS,
-                                   fragment_correction != 0, window_length, quality_threshold, true, 3, -5, -4, 0));
+                                   fragment_correction != 0, window_length, quality_threshold, true, 3, -5, -4, {0}));
     h->polisher->build_windows(ovl);
+    h->overlaps = std::move(ovl);
     return h;
 }
 
@@ -615,14 +704,15 @@ extern "C" void* rp_mirror_polisher_open_with_bp(uint32_t n_seq, const char* bas
 extern "C" void* rp_mirror_polisher_open_files(const char* reads, const char* overlaps, const char* targets,
                                                int fragment_correction, uint32_t window_length, double quality_threshold,
                                                double error_threshold, int trim, int8_t match, int8_t mismatch, int8_t gap,
-                                               uint32_t device, int resident_reads, char* err, uint32_t err_cap) {
+                                               const uint32_t* devices, uint32_t n_devices, int resident_reads, char* err,
+                                               uint32_t err_cap) {
     using namespace racon_b200;
     try {
         std::unique_ptr<PolHandle> h(new PolHandle());
         h->input.reset(new InputSet(load_input(reads, overlaps, targets, fragment_correction != 0, error_threshold)));
         h->polisher.reset(new Polisher(h->input->views(), h->input->targets_size, h->input->window_type,
                                        fragment_correction != 0, window_length, quality_threshold, trim != 0, match,
-                                       mismatch, gap, device));
+                                       mismatch, gap, std::vector<uint32_t>(devices, devices + n_devices)));
         h->polisher->use_resident_reads(resident_reads != 0);
         h->polisher->initialize(h->input->overlaps);
         return h.release();
@@ -633,6 +723,25 @@ extern "C" void* rp_mirror_polisher_open_files(const char* reads, const char* ov
         }
         return nullptr;
     }
+}
+
+/* The breaking points initialize() found: those of overlap i are the (t, q) pairs pts[2 off[i]] .. pts[2 off[i + 1]]
+ * (off: one entry per overlap + 1).  Returns the number of points; off / pts NULL = count only. */
+extern "C" uint64_t rp_mirror_polisher_breaking_points(void* hv, uint64_t* off, uint32_t* pts) {
+    const auto& overlaps = static_cast<PolHandle*>(hv)->all_overlaps();
+    uint64_t n = 0;
+    for (size_t i = 0; i < overlaps.size(); ++i) {
+        if (off) off[i] = n;
+        for (const auto& p : overlaps[i].breaking_points()) {
+            if (pts) {
+                pts[2 * n] = p.first;
+                pts[2 * n + 1] = p.second;
+            }
+            ++n;
+        }
+    }
+    if (off) off[overlaps.size()] = n;
+    return n;
 }
 
 /* failed[0] = overlaps, failed[1] = windows the device could not finish (Polisher::failed_overlaps/failed_windows) */
@@ -737,6 +846,25 @@ extern "C" uint32_t rp_mirror_polisher_stream_fasta(void* hv, int drop_unpolishe
 }
 
 extern "C" void rp_mirror_polisher_close(void* hv) { delete static_cast<PolHandle*>(hv); }
+
+/* Host-only test hook of the stitch cursor (InOrderStitcher): n_ranges contiguous ranges of counts[r] windows finish in
+ * the order `completion` (a permutation of 0 .. n_ranges - 1).  order[i] = the i-th window emitted, step[i] = the position
+ * in `completion` of the range whose finish emitted it.  Returns the number of windows emitted. */
+extern "C" uint64_t rp_mirror_stitch_order(uint32_t n_ranges, const uint32_t* counts, const uint32_t* completion,
+                                           uint64_t* order, uint32_t* step) {
+    std::vector<uint64_t> first(n_ranges + 1, 0);
+    for (uint32_t r = 0; r < n_ranges; ++r) first[r + 1] = first[r] + counts[r];
+    racon_b200::InOrderStitcher stitcher(first[n_ranges]);
+    uint64_t n = 0;
+    for (uint32_t i = 0; i < n_ranges; ++i) {
+        const uint32_t r = completion[i];
+        stitcher.finish(first[r], counts[r], [&](size_t w) {
+            order[n] = w;
+            step[n++] = i;
+        });
+    }
+    return n;
+}
 
 /* host-only: one FASTA record; returns its length (out may be NULL to size it) */
 extern "C" uint64_t rp_mirror_format_fasta(const char* name, const char* tags, const char* data, uint64_t data_len,

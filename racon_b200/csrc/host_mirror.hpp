@@ -95,6 +95,9 @@ public:
      * launch() queues H2D + kernel + D2H on the object's stream and returns, collect() waits and reads back */
     void launch();
     const std::vector<bool>& collect();
+    /* true when the launched batch has finished on the device (rp_poa_query): collect() then does not wait for the
+     * kernel */
+    bool ready();
     void reset();
     uint32_t getBatchID() const { return bid_; }
     /* From now on windows that know the origin of all their pieces (Window::origins) are added by reference into
@@ -196,12 +199,39 @@ struct PolishedSequence {
 /* One FASTA record as racon's main prints a polished sequence (src/main.cpp:159-161): ">name tags\ndata\n". */
 std::string format_fasta(const std::string& target_name, const PolishedSequence& s);
 
+/* The stitch cursor of the polisher: ranges of windows [first, first + count) finish in any order, and emit(w) is called
+ * once for every window, in window order, as soon as it and every window before it have finished.  A range that
+ * finishes early waits (its windows keep their consensus) until the ranges before it are in. */
+class InOrderStitcher {
+public:
+    explicit InOrderStitcher(size_t n_windows) : finished_(n_windows, 0) {}
+    template <typename Emit>
+    void finish(size_t first, size_t count, Emit&& emit) {
+        for (size_t w = first; w < first + count; ++w) finished_[w] = 1;
+        while (cursor_ < finished_.size() && finished_[cursor_]) emit(cursor_++);
+    }
+    size_t cursor() const { return cursor_; }   // windows emitted so far
+
+private:
+    std::vector<uint8_t> finished_;
+    size_t cursor_ = 0;
+};
+
+/* The polisher runs its two device stages on a list of devices: one lane per entry (the same device may appear more than
+ * once: {0, 0} = two lanes on one GPU).  The aligner has one batch object per lane, the consensus two; one host thread
+ * hands every idle object the next contiguous range of overlaps / windows, launches it asynchronously and collects
+ * whichever object has finished (rp_*_query), waiting for the oldest one only when none has — so devices that do not
+ * finish in step never hold each other up.  Results are per overlap / per window and the stitch cursor
+ * (InOrderStitcher) restores window order, so the output does not depend on the devices, their number or the order in
+ * which they finish: a list of one device is the single-GPU polisher.  Every distinct device holds one copy of the
+ * read store, shared by the lanes on it. */
 class Polisher {
 public:
-    /* sequences: the targets first (targets_size of them), then the reads — the order racon::Polisher::sequences_ has */
+    /* sequences: the targets first (targets_size of them), then the reads — the order racon::Polisher::sequences_ has;
+     * devices: CUDA device indices, one lane each (not empty; each below rp_device_count() when a device is visible) */
     Polisher(std::vector<SequenceView> sequences, uint64_t targets_size, WindowType window_type, bool fragment_correction,
              uint32_t window_length, double quality_threshold, bool trim, int8_t match, int8_t mismatch, int8_t gap,
-             uint32_t device);
+             std::vector<uint32_t> devices);
     ~Polisher();
     /* Device-resident reads: every sequence is uploaded once (rp_reads_create, at first use) and both device stages name
      * their inputs instead of copying them — the aligner its two spans per overlap (rp_aln_add_overlap_ref), the consensus
@@ -213,8 +243,9 @@ public:
     void build_windows(const std::vector<Overlap>& overlaps);
     void polish(std::vector<PolishedSequence>& dst, bool drop_unpolished_sequences);
     /* Streaming form (polisher.cpp:504-537 + main.cpp:159-161 as a consumer overlapped with the compute): two batch
-     * objects stay in flight; while one runs on the GPU the other's finished windows are stitched in window order, and
-     * `sink` gets every polished sequence the moment its last window is collected (e.g. a FASTA writer).  `memory` =
+     * objects per lane stay in flight; while they run on the GPUs the finished windows are stitched in window order, and
+     * `sink` gets every polished sequence the moment its last window is stitched (e.g. a FASTA writer); stitched windows
+     * are released.  `memory` =
      * device budget per batch object (0 = library default), `banded` = racon -b.  `resident_reads`: upload every sequence
      * once (rp_reads) and add the windows by reference — layer extraction on the device, no host copy of layer bytes. */
     void polish_streaming(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
@@ -233,6 +264,15 @@ private:
     const Polisher& operator=(const Polisher&) = delete;
     const char* reverse_complement(uint32_t id);
     const char* reverse_quality(uint32_t id);
+    /* the aligner lanes of find_overlap_breaking_points over overlaps[todo[..]] */
+    void align(std::vector<Overlap>& overlaps, const std::vector<size_t>& todo, uint32_t longest);
+    /* the one batch loop + stitch of polish() and polish_streaming(); `release`: drop every window once stitched.  A
+     * hard error in either stage destroys its batch objects and the read stores before the process exits. */
+    void consensus(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
+                   size_t memory, bool banded, bool resident_reads, bool release);
+    void consensus_lanes(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
+                         size_t memory, bool banded, bool resident_reads, bool release);
+    void release_read_stores();
 
     std::vector<SequenceView> sequences_;
     uint64_t targets_size_;
@@ -242,15 +282,15 @@ private:
     double quality_threshold_;
     bool trim_;
     int8_t match_, mismatch_, gap_;
-    uint32_t device_;
+    std::vector<uint32_t> devices_;
     std::string dummy_quality_;
     std::vector<std::string> reverse_complement_, reverse_quality_;
     std::vector<uint32_t> targets_coverages_;
     std::vector<std::shared_ptr<Window>> windows_;
     std::vector<size_t> failed_overlaps_, failed_windows_;
     bool resident_reads_ = false;
-    rp_reads* store_ = nullptr;
-    const rp_reads* read_store();
+    std::vector<std::pair<uint32_t, rp_reads*>> stores_;   // (device, store): one per distinct device, made at first use
+    const rp_reads* read_store(uint32_t device);
 };
 
 }  // namespace racon_b200

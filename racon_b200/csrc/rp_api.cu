@@ -150,6 +150,17 @@ rp_status set_stream(StreamOwner* o, void* cuda_stream) {
     return RP_OK;
 }
 
+/* rp_*_query: has the work queued on the object's stream by its last run finished? (`launched`: the object's flag) */
+rp_status query_stream(StreamOwner* o, bool launched) {
+    if (!o) return fail(RP_ERR_INVALID, "null object");
+    if (!launched) return fail(RP_ERR_STATE, "query before run");
+    RP_CUDA(cudaSetDevice(o->device));
+    const cudaError_t e = cudaStreamQuery(o->stream);
+    if (e == cudaErrorNotReady) return RP_NOT_READY;
+    RP_CUDA(e);
+    return RP_OK;
+}
+
 constexpr int kWarpsPerBlock = 4;
 constexpr uint32_t kBandPaysFromWindowLength = 768;   // rows of two or more 512-column chunks
 
@@ -413,6 +424,7 @@ const char* rp_strerror(rp_status s) {
     switch (s) {
         case RP_OK: return "ok";
         case RP_BATCH_FULL: return "batch full";
+        case RP_NOT_READY: return "not ready: the last run is still in flight";
         case RP_ERR_INVALID: return "invalid argument or malformed window";
         case RP_ERR_CUDA: return "CUDA error";
         case RP_ERR_NOMEM: return "out of memory";
@@ -1061,6 +1073,8 @@ rp_status rp_poa_sync(rp_poa* p) {
     return RP_OK;
 }
 
+rp_status rp_poa_query(rp_poa* p) { return query_stream(p, p && p->launched); }
+
 static rp_status ensure_results(rp_poa* p) {
     if (!p) return fail(RP_ERR_INVALID, "null object");
     if (!p->downloaded) return fail(RP_ERR_STATE, "fetch before run/download");
@@ -1426,6 +1440,8 @@ rp_status rp_aln_sync(rp_aln* a) {
     return RP_OK;
 }
 
+rp_status rp_aln_query(rp_aln* a) { return query_stream(a, a && a->launched); }
+
 rp_status rp_aln_fetch_cigar(rp_aln* a, uint32_t i, const char** cigar, uint32_t* len, int32_t* edit_distance,
                              uint32_t* status) {
     if (!a) return fail(RP_ERR_INVALID, "null object");
@@ -1436,7 +1452,9 @@ rp_status rp_aln_fetch_cigar(rp_aln* a, uint32_t i, const char** cigar, uint32_t
     }
     if (i >= rp_aln_size(a)) return fail(RP_ERR_INVALID, "overlap index out of range");
     uint32_t st = a->pre_status[i] ? a->pre_status[i] : a->h_status.data[i];
-    if (!a->cigar_built[i]) {
+    /* the text is built on the first call that asks for it: a caller after the status alone (the polisher, which takes
+     * the breaking points) pays nothing per run */
+    if ((cigar || len) && !a->cigar_built[i]) {
         std::string& c = a->cigars[i];
         if (st == RP_ALN_OK) {
             const uint32_t* r = a->h_runs.data + a->run_off.data[i];
