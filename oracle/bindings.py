@@ -62,6 +62,8 @@ def oracle_lib():
         lib.oracle_graph_shape.restype = C.c_int
         lib.oracle_graph_shape.argtypes = _CONS_ARGS[:13] + [C.c_uint32, C.c_void_p, C.c_uint32] + [C.c_void_p, C.c_uint32] + \
             [C.c_void_p] * 3
+        lib.oracle_poa_set_tie_rules.restype = None
+        lib.oracle_poa_set_tie_rules.argtypes = [C.c_uint32]
         lib.oracle_poa_trace_begin.restype = None
         lib.oracle_poa_trace_begin.argtypes = []
         lib.oracle_poa_trace_end.restype = C.c_uint64
@@ -117,6 +119,31 @@ def oracle_consensus(ws, m=3, x=-5, g=-4, window_length=500, trim=True, threads=
     if want_coverage:
         return cons, pol, secs, [cov[w, :len(cons[w])].copy() for w in range(n)]
     return cons, pol, secs
+
+
+# spoa's tie rules, one bit each: oracle_poa_set_tie_rules(bit) replaces that rule by its opposite
+TIE_RULES = {
+    "first_in_edge_diagonal": 1 << 0,   # traceback, diagonal step: predecessors in in-edge order, the first match wins
+    "vertical_before_horizontal": 1 << 1,
+    "first_tied_sink": 1 << 2,          # equal best scores in the last column: the first sink in rank order wins
+    "bundle_tie_le": 1 << 3,            # heaviest bundle, equal edge weights: scores[pred] <= scores[tail] takes the tail
+    "first_best_node": 1 << 4,          # heaviest bundle: the strict maximum keeps the first best node in rank order
+}
+
+
+def oracle_poa_set_tie_rules(mask):
+    """TESTS ONLY: every later oracle call breaks ties with the opposite of each rule set in `mask` (TIE_RULES); 0, the
+    default, is spoa.  It exists to show that a test's windows reach a rule, never to check a result."""
+    oracle_lib().oracle_poa_set_tie_rules(mask)
+
+
+def oracle_consensus_with_tie_rules(ws, mask, *args, **kw):
+    """oracle_consensus with the tie rules of `mask` flipped, then spoa's rules again"""
+    oracle_poa_set_tie_rules(mask)
+    try:
+        return oracle_consensus(ws, *args, **kw)
+    finally:
+        oracle_poa_set_tie_rules(0)
 
 
 def oracle_matrix_ranges(ws, m=3, x=-5, g=-4, window_length=500, trim=True):

@@ -45,6 +45,28 @@ Stats g_stats;
 bool g_trace_on = false;
 std::vector<int64_t> g_trace;
 
+/* oracle_poa_set_tie_rules: TESTS ONLY.  Each set bit replaces one of spoa's tie rules with its opposite, so that a test
+ * can show that its windows reach the rule (the consensus changes); 0, the default, is spoa. */
+enum : uint32_t {
+    kTieLastInEdgeDiag = 1u << 0,    // traceback, diagonal step: the last explaining in-edge instead of the first
+    kTieHorizFirst = 1u << 1,        // traceback: horizontal step before vertical
+    kTieLastSink = 1u << 2,          // last tied sink in rank order instead of the first
+    kTieBundleStrict = 1u << 3,      // heaviest bundle, equal weights: scores[pred] < scores[tail] instead of <=
+    kTieLastBestNode = 1u << 4,      // heaviest bundle: the last best node in rank order instead of the first
+};
+std::atomic<uint32_t> g_tie_rules{0};
+
+bool tie_rule(uint32_t bit) { return (g_tie_rules.load(std::memory_order_relaxed) & bit) != 0; }
+
+/* the heaviest-bundle choice of graph.cpp:448-449 / 500-501 between the current predecessor and tail t */
+bool heavier_edge(int64_t weight, int64_t score, int64_t pred_score, int64_t tail_score) {
+    if (score != weight) return score < weight;
+    return tie_rule(kTieBundleStrict) ? pred_score < tail_score : pred_score <= tail_score;
+}
+
+/* graph.cpp:454-456 / 506-508: is `s` a new best node score over `best`? */
+bool new_best(int64_t best, int64_t s) { return tie_rule(kTieLastBestNode) ? best <= s : best < s; }
+
 struct Edge {
     uint32_t tail, head;
     int64_t weight;
@@ -219,14 +241,13 @@ struct Graph {
             for (uint32_t e : inedges[it]) {
                 uint32_t t = edges[e].tail;
                 if (scores[t] == -1) continue;
-                if (scores[it] < edges[e].weight ||
-                    (scores[it] == edges[e].weight && scores[pred[it]] <= scores[t])) {
+                if (heavier_edge(edges[e].weight, scores[it], pred[it] >= 0 ? scores[pred[it]] : 0, scores[t])) {
                     scores[it] = edges[e].weight;
                     pred[it] = t;
                 }
             }
             if (pred[it] >= 0) scores[it] += scores[pred[it]];
-            if (max < 0 || scores[max] < scores[it]) max = it;
+            if (max < 0 || new_best(scores[max], scores[it])) max = it;
         }
         return max;
     }
@@ -241,14 +262,13 @@ struct Graph {
             for (uint32_t it : rank_to_node) {
                 for (uint32_t e : inedges[it]) {
                     uint32_t t = edges[e].tail;
-                    if (scores[it] < edges[e].weight ||
-                        (scores[it] == edges[e].weight && scores[pred[it]] <= scores[t])) {
+                    if (heavier_edge(edges[e].weight, scores[it], pred[it] >= 0 ? scores[pred[it]] : 0, scores[t])) {
                         scores[it] = edges[e].weight;
                         pred[it] = t;
                     }
                 }
                 if (pred[it] >= 0) scores[it] += scores[pred[it]];
-                if (max < 0 || scores[max] < scores[it]) max = it;
+                if (max < 0 || new_best(scores[max], scores[it])) max = it;
             }
             if (!outedges[max].empty()) {
                 std::vector<uint32_t> node_to_rank(n, 0);
@@ -380,6 +400,7 @@ struct Engine {
                     n_tied = 1;
                 } else if (max_score == Hr[W - 1]) {
                     ++n_tied;
+                    if (tie_rule(kTieLastSink)) max_i = i;
                 }
             }
         }
@@ -410,7 +431,9 @@ struct Engine {
                 const auto& in = graph.inedges[v];
                 int32_t mc = (graph.code[v] == static_cast<uint8_t>(seq[j - 1])) ? m : x;
                 size_t np = std::max<size_t>(1, in.size());
-                for (size_t p = 0; p < np && !found; ++p) {
+                const bool last_first = tie_rule(kTieLastInEdgeDiag);
+                for (size_t k = 0; k < np && !found; ++k) {
+                    size_t p = last_first ? np - 1 - k : k;
                     uint32_t pi = in.empty() ? 0 : node_to_rank[graph.edges[in[p]].tail] + 1;
                     if (Hij == H[pi * W + (j - 1)] + mc) {
                         prev_i = pi;
@@ -418,6 +441,12 @@ struct Engine {
                         found = true;
                     }
                 }
+            }
+            const bool horiz_first = tie_rule(kTieHorizFirst);
+            if (!found && horiz_first && j != 0 && Hij == H[i * W + j - 1] + g) {
+                prev_i = i;
+                prev_j = j - 1;
+                found = true;
             }
             if (!found && i != 0) {
                 const auto& in = graph.inedges[r2n[i - 1]];
@@ -431,7 +460,7 @@ struct Engine {
                     }
                 }
             }
-            if (!found && Hij == H[i * W + j - 1] + g) {
+            if (!found && !horiz_first && Hij == H[i * W + j - 1] + g) {
                 prev_i = i;
                 prev_j = j - 1;
                 found = true;
@@ -661,6 +690,9 @@ void oracle_poa_stats(uint64_t* out) {
     out[10] = g_stats.far_pred_rows.exchange(0);
     out[11] = g_stats.pred_rows.exchange(0);
 }
+
+/* TESTS ONLY: replace spoa's tie rules by the ones set in `mask` (kTie* above) for every later call; 0 restores spoa. */
+void oracle_poa_set_tie_rules(uint32_t mask) { g_tie_rules = mask; }
 
 void oracle_poa_trace_begin(void) {
     g_trace.clear();
