@@ -155,10 +155,19 @@ rp_status rp_poa_reset(rp_poa* p);        /* CUDABatchProcessor::reset (cudabatc
 rp_status rp_poa_set_stream(rp_poa* p, void* cuda_stream);   /* use the caller's cudaStream_t */
 /* info[0] kernel launches so far, [1] last H2D bytes, [2] last D2H bytes, [3] worker warps,
  * [4] scratch bytes per warp; with counters enabled: [5] alignments done, [6] DP cells sum (L+1)(N+1),
- * [7] predecessor cells sum (L+1)*E (E = sum over rows of max(1, in-degree)) — SURVEY.md §8(d) byte model */
+ * [7] predecessor cells sum (L+1)*E (E = sum over rows of max(1, in-degree)) — SURVEY.md §8(d) byte model.
+ * L = read length, N = graph rows of the alignment (the subgraph's for a partial-span layer); an alignment accepted
+ * inside the band counts the band width in place of L+1.
+ * [5]-[7] are per launch, not cumulative: every rp_poa_launch (and so every rp_poa_run) starts them from zero, and
+ * rp_poa_download reads back those of the launch before it (all three 0 when counters were off at that download, or
+ * the batch had no GPU window).  They count the first pass only: the escalation pass rp_poa_sync runs for windows over
+ * a first-pass limit is not counted, so such a window contributes the alignments it finished before it failed the
+ * first pass (none, when its backbone is over the node budget or its first layer over the length limit).  Windows of
+ * fewer than 3 sequences and windows over the alphabet limit never reach the device and count nothing. */
 rp_status rp_poa_info(rp_poa* p, uint64_t info[8]);
 rp_status rp_poa_enable_counters(rp_poa* p, int on);
-/* racon -b / --cuda-banded-alignment (createCUDABatch's `banded`, cudabatch.cpp:56-59): after a run,
+/* racon -b / --cuda-banded-alignment (createCUDABatch's `banded`, cudabatch.cpp:56-59): after a run (counts of the
+ * last launch's first pass, like rp_poa_info's [5]-[7]),
  * info[0] = 1 when the object is banded, [1] alignments tried inside the band, [2] alignments whose band result
  * was refused by the device-side check and that were redone with the full matrix on the device, [3] band width
  * in columns, [4] (only with the environment variable RP_BAND_AUDIT=1, a test mode that recomputes every accepted

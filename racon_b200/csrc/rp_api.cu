@@ -953,7 +953,8 @@ rp_status rp_poa_launch(rp_poa* p) {
     RP_CUDA(cudaSetDevice(p->device));
     if (p->P.n_windows > 0) {
         RP_CUDA(cudaMemsetAsync(p->d_head.p, 0, 4, p->stream));
-        RP_CUDA(cudaMemsetAsync(static_cast<uint8_t*>(p->d_stats.p) + 128, 0, 32, p->stream));
+        /* the DP counters [0, 64) and the band counters [128, 160) count this launch alone */
+        RP_CUDA(cudaMemsetAsync(p->d_stats.p, 0, 160, p->stream));
         p->P.stats = p->counters ? static_cast<uint64_t*>(p->d_stats.p) : nullptr;
         p->P.band_stats = reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(p->d_stats.p) + 128);
         const uint32_t need_blocks = (p->P.n_windows + p->groups_per_block - 1) / p->groups_per_block;
@@ -987,8 +988,10 @@ rp_status rp_poa_download(rp_poa* p) {
         if (s != RP_OK) return s;
         d2h = p->batch.out_total * 3 + static_cast<uint64_t>(n) * 8;
     }
-    if (p->counters)
+    if (p->counters && n > 0)
         RP_CUDA(cudaMemcpyAsync(p->h_stats, p->d_stats.p, 64, cudaMemcpyDeviceToHost, p->stream));
+    else
+        std::memset(p->h_stats, 0, sizeof(p->h_stats));
     if (p->banded && n > 0)
     {
         RP_CUDA(cudaMemcpyAsync(p->h_band, static_cast<uint8_t*>(p->d_stats.p) + 128, 32, cudaMemcpyDeviceToHost,
