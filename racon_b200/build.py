@@ -5,6 +5,7 @@
                            the reference interface restated; reads_io: FASTA/FASTQ/PAF/MHAP/SAM input) + the rp_mirror_* hooks tests/ and
                            bench.py drive it with;
                            links against the product, never part of it
+  racon_b200             — the command line over the host layer: racon's arguments in, polished FASTA on stdout
   libracon_synth.so      — synthetic window generator (bench/test input maker, no CUDA)
   libracon_sim.so   — TEST-ONLY host simulation of the device code (tests/ only)
   simapi/libracon_b200.so, simapi/libracon_b200_host.so — TEST-ONLY: the C ABI and the host layer over a simulated CUDA
@@ -81,6 +82,22 @@ def build_cuda(force=False, verbose=False):
         if verbose:
             print(log)
     build_host(force)
+    build_cli(force)
+    return out
+
+
+def build_cli(force=False):
+    """The racon_b200 command line (racon's arguments, polished FASTA on stdout) over the host layer; finds both libraries
+    next to itself ($ORIGIN), so it runs without Python."""
+    os.makedirs(LIBDIR, exist_ok=True)
+    out = os.path.join(LIBDIR, "racon_b200")
+    src = os.path.join(CSRC, "racon_main.cpp")
+    deps = [src, os.path.join(CSRC, "host_mirror.hpp"), os.path.join(CSRC, "reads_io.hpp"),
+            os.path.join(ROOT, "include", "racon_b200.h"), os.path.join(LIBDIR, "libracon_b200.so"),
+            os.path.join(LIBDIR, "libracon_b200_host.so")]
+    if force or _newer(out, deps):
+        _run(["g++", "-std=c++17", "-O2", "-I", os.path.join(ROOT, "include"), "-I", CSRC, "-o", out, src,
+              "-L", LIBDIR, "-lracon_b200_host", "-lracon_b200", "-Wl,-rpath,$ORIGIN"])
     return out
 
 
