@@ -141,7 +141,8 @@ rp_status rp_poa_launch(rp_poa* p);
 rp_status rp_poa_download(rp_poa* p);
 
 /* Window::consensus() + the bool generate_consensus returns (window.cpp:65-149); coverage = per-base
- * coverage of the returned consensus (Graph::GenerateConsensus summary, graph.cpp:377-398). */
+ * coverage of the returned consensus (Graph::GenerateConsensus summary, graph.cpp:377-398), saturated at 65 535
+ * (cudapoa's uint16).  The device counts sequences through a node in 32 bits, and the trim compares the exact sum. */
 rp_status rp_poa_fetch(rp_poa* p, uint32_t i, const char** consensus, uint32_t* len, const uint16_t** coverage,
                        int* polished);
 rp_status rp_poa_window_status(rp_poa* p, uint32_t i, uint32_t* status);

@@ -86,7 +86,7 @@ RP_HD SlotLayout make_layout(const PoaLimits& L) {
     s.flags = take(n);
     s.in_cnt = take(n);
     s.al_cnt = take(n);
-    s.cov = take(n * 2);
+    s.cov = take(n * 4);
     s.in_tail = take(n * L.ki * 2);
     s.in_w = take(n * L.ki * 4);
     s.al = take(n * L.ka * 2);
@@ -380,7 +380,8 @@ struct PoaWarp {
     int lane;
     /* graph (HBM) */
     uint8_t *code, *flags, *in_cnt, *al_cnt, *member, *has_out_sub, *marks;
-    uint16_t *cov, *in_tail, *al, *order, *order_nxt, *rank_of, *dp_order, *dp_rank, *pred_ovf, *aln, *cur, *cpred,
+    uint32_t* cov;       // per node: sequences through it (spoa's Node::Coverage, a uint32 there too)
+    uint16_t *in_tail, *al, *order, *order_nxt, *rank_of, *dp_order, *dp_rank, *pred_ovf, *aln, *cur, *cpred,
         *sorder, *srank, *stack;
     int32_t* in_w;
     Rec* rec;
@@ -411,7 +412,7 @@ struct PoaWarp {
         flags = slot + y.flags;
         in_cnt = slot + y.in_cnt;
         al_cnt = slot + y.al_cnt;
-        cov = reinterpret_cast<uint16_t*>(slot + y.cov);
+        cov = reinterpret_cast<uint32_t*>(slot + y.cov);
         in_tail = reinterpret_cast<uint16_t*>(slot + y.in_tail);
         in_w = reinterpret_cast<int32_t*>(slot + y.in_w);
         al = reinterpret_cast<uint16_t*>(slot + y.al);
@@ -1932,7 +1933,7 @@ struct PoaWarp {
 #pragma unroll
             for (int u = 0; u < kU; ++u) {
                 if (c[u] == kNone) continue;
-                if (len >= 2) cov[c[u]] = static_cast<uint16_t>(cv[u] + 1);
+                if (len >= 2) cov[c[u]] = cv[u] + 1;
                 if (pv[u] == kNone) continue;
                 uint32_t q = 0;
                 for (; q < ni[u]; ++q) {
@@ -2109,7 +2110,8 @@ struct PoaWarp {
         }
         clen = shfl(clen, 0);
         syncwarp();
-        /* coverage (graph.cpp:388-394): node + its aligned nodes, counted as sequences through the node */
+        /* coverage (graph.cpp:388-394): node + its aligned nodes, counted as sequences through the node.  The trim
+         * compares the exact 32-bit sum; only the per-base output (uint16, cudapoa's type) saturates at 65 535. */
         uint32_t thr = (n_seq - 1) / 2;
         uint32_t first = 0xffffffffu, last = 0;
         for (uint32_t k = lane; k < clen; k += G) {
@@ -2117,8 +2119,7 @@ struct PoaWarp {
             uint32_t c = cov[v];
             uint32_t na = al_cnt[v];
             for (uint32_t q = 0; q < na; ++q) c += cov[al[v * ka + q]];
-            if (c > 0xffffu) c = 0xffffu;
-            dp_rank[k] = static_cast<uint16_t>(c);  // dp_rank is idle here: per-base coverage scratch
+            dp_rank[k] = static_cast<uint16_t>(c > 0xffffu ? 0xffffu : c);  // dp_rank is idle here: coverage scratch
             if (c >= thr) {
                 if (k < first) first = k;
                 if (k + 1 > last) last = k + 1;

@@ -6,19 +6,23 @@ sample files (tests/golden/data) over racon's option set:
   -m 5 -x -4 -g -8 and medaka's recommended scores -m 8 -x -6 -g -8;
   on the fragment-correction FASTQ + PAF case: -f -u, -f --no-trimming -w 300 and -f -u -m 1 -x -1 -g -1 (the run
   of racon's own tests).
+Generated inputs, whose files are written by a function of the test suite and never committed (the case records the
+function as "generator"): a deep amplicon, 66 000 reads through one window (tests/test_gpu_poa_depth.py).
 Per case: the options and the three files, the record count, the total bases, the md5 of stdout
 and the header lines (name + tags).  racon's output does not depend on its thread count, so it runs with -t 8 here.
-Stored in tests/golden/cli_cases.json.  Run on a machine with the reference sources:  python tests/golden/make_cli_cases.py"""
+Stored in tests/golden/cli_cases.json.  Run on a machine with the reference sources:  python tests/golden/make_cli_cases.py
+[case ...] (only the named cases are remade, the others are kept)"""
 import hashlib
 import json
 import os
 import subprocess
 import sys
+import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 from oracle import refcli  # noqa: E402
-from tests import util  # noqa: E402
+from tests import test_gpu_poa_depth as depth, util  # noqa: E402
 from tests.test_reads_io import CASES  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden", "cli_cases.json")
@@ -55,6 +59,10 @@ def cases():
     return out
 
 
+# name: (options, function that writes the three files into a directory and returns their paths)
+GENERATED = {"deep_amplicon": ([], depth.write_deep_amplicon)}
+
+
 def summary(stdout):
     """count, bases, md5 of the whole stdout, header lines (without '>') of a FASTA with one line per sequence"""
     lines = stdout.split(b"\n")
@@ -65,22 +73,37 @@ def summary(stdout):
             "names": [n[1:].decode() for n in names]}
 
 
-def main():
+def _run(exe, name, opts, paths):
+    r = subprocess.run([exe] + opts + ["-t", "8"] + paths, stdout=subprocess.PIPE, stderr=subprocess.DEVNULL,
+                       timeout=3600)
+    assert r.returncode == 0, (name, r.returncode)
+    rec = summary(r.stdout)
+    print("%-34s %3d records %9d bases  %s" % (name, rec["count"], rec["bases"], rec["md5"]))
+    return rec
+
+
+def main(only=()):
     exe = refcli.build_refcli()
     assert exe, "the reference's command line needs the reference sources"
     data = util.sample_data_dir()
     fixture = {}
+    if only:
+        with open(OUT) as f:
+            fixture = json.load(f)
     for name, (opts, files) in cases().items():
-        r = subprocess.run([exe] + opts + ["-t", "8"] + [os.path.join(data, f) for f in files],
-                           stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, timeout=3600)
-        assert r.returncode == 0, (name, r.returncode)
-        fixture[name] = dict({"options": opts, "files": files}, **summary(r.stdout))
-        print("%-34s %3d records %9d bases  %s" % (name, fixture[name]["count"], fixture[name]["bases"],
-                                                   fixture[name]["md5"]))
+        if not only or name in only:
+            fixture[name] = dict({"options": opts, "files": files},
+                                 **_run(exe, name, opts, [os.path.join(data, f) for f in files]))
+    for name, (opts, gen) in GENERATED.items():
+        if not only or name in only:
+            with tempfile.TemporaryDirectory() as d:
+                paths = gen(d)
+                fixture[name] = dict({"options": opts, "generator": "%s.%s" % (gen.__module__, gen.__name__),
+                                      "files": [os.path.basename(p) for p in paths]}, **_run(exe, name, opts, paths))
     with open(OUT, "w") as f:
         json.dump(fixture, f, indent=1)
         f.write("\n")
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1:])

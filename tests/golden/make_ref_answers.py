@@ -1,6 +1,7 @@
 """Generates tests/golden/ref_answers.json: what the UNMODIFIED reference (oracle/_ref, built by oracle/Makefile) answers
 on the inputs of tests/test_oracle.py (spoa consensus through Window::generate_consensus), on one seed of each tie-rich
-window generator of tests/test_gpu_poa_ties.py, and on those of tests/test_myers_oracle.py (edlib CIGARs), so that those comparisons also run where oracle/_ref is not built.  Run where it is:
+window generator of tests/test_gpu_poa_ties.py, on three deep windows of the coverage ladder of tests/test_gpu_poa_depth.py,
+and on those of tests/test_myers_oracle.py (edlib CIGARs), so that those comparisons also run where oracle/_ref is not built.  Run where it is:
     python tests/golden/make_ref_answers.py"""
 import json
 import os
@@ -10,7 +11,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, ROOT)
 
 from oracle import bindings as ob  # noqa: E402
-from tests import test_gpu_poa_ties as tt, test_myers_oracle as tm, test_oracle as to, util  # noqa: E402
+from tests import test_gpu_poa_depth as td, test_gpu_poa_ties as tt, test_myers_oracle as tm, test_oracle as to, util  # noqa: E402
 
 
 def main():
@@ -29,6 +30,8 @@ def main():
         case = tt.pinned_case(kind)
         for scores in tt.SCORES:
             poa[tt.pinned_key(kind, scores)] = util.consensus_answer(*case(ob.ref_consensus, scores))
+    for n in td.PINNED:
+        poa[td.pinned_key(n)] = util.consensus_answer(*td.pinned_case(n)(ob.ref_consensus))
     edlib = {}
     for n, err, count in tm.TRACEBACK:
         edlib["traceback/%d" % n] = [util.cigar_answer(ob.ref_edlib_cigar(q, t)) for q, t in tm.traceback_pairs(n, err, count)]
