@@ -57,6 +57,8 @@ enum { RP_WINDOW_NGS = 0, RP_WINDOW_TGS = 1 }; /* racon::WindowType, src/window.
 const char* rp_strerror(rp_status s);
 const char* rp_last_error(void);          /* thread-local text of the last hard error */
 int rp_device_count(void);                /* cudaGetDeviceCount; <= 0 when no device (cudapolisher.cpp:48) */
+/* cudaMemGetInfo on `device`: the bytes free and in all (what the batch objects size their defaults from) */
+rp_status rp_device_memory(int device, uint64_t* free_bytes, uint64_t* total_bytes);
 const char* rp_version(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -93,12 +95,16 @@ rp_status rp_poa_add_window(rp_poa* p, uint32_t n_seq, const char* const* seq, c
  * rp_reads_create: data[i] / length[i] = sequence i (targets and reads, any order); quality[i] NULL (or quality NULL) =
  * no qualities.  The host arrays must stay valid while the store is alive (backbone copies of windows with < 3 sequences
  * and the rare exact alphabet scan read them).  One store can serve any number of batch objects on the same device, on
- * any of their streams: nothing writes to a store after rp_reads_create has returned (its upload is complete by then). */
+ * any of their streams: nothing writes to a store after rp_reads_create has returned (its upload is complete by then).
+ * A sequence given with length 0 (its data may then be NULL) is absent: it costs nothing, and a window piece or an
+ * overlap that names it with a non-empty span is refused with RP_ERR_INVALID.  A store can so hold a subset of a
+ * sequence table under the table's own ids. */
 typedef struct rp_reads rp_reads;
 rp_status rp_reads_create(rp_reads** out, int device, uint32_t n_seqs, const char* const* data,
                           const char* const* quality, const uint32_t* length);
 void rp_reads_destroy(rp_reads* r);
-/* device bytes the store occupies */
+/* Device bytes the store occupies, exactly: (sum of length[i] + 16) bytes of bases, and the same again for qualities
+ * when any sequence of non-zero length has a quality string.  Callers size their stores with this rule. */
 uint64_t rp_reads_bytes(const rp_reads* r);
 
 /* rp_poa_add_window with the pieces named instead of passed: piece k = length[k] bases of sequence seq_id[k] starting at

@@ -29,6 +29,7 @@ SIGNATURES = {
     "rp_strerror": (_str, [_st]),
     "rp_last_error": (_str, []),
     "rp_device_count": (_int, []),
+    "rp_device_memory": (_st, [_int, _vp, _vp]),
     "rp_version": (_str, []),
     "rp_poa_create": (_st, [C.POINTER(_vp), _int, _size, _i8, _i8, _i8, _int, _u32, _u32]),
     "rp_poa_destroy": (None, [_vp]),
@@ -93,6 +94,11 @@ HOST_SIGNATURES = {
     "rp_mirror_polisher_failed": (None, [_vp, _vp]),
     "rp_mirror_polisher_breaking_points": (_u64, [_vp, _vp, _vp]),
     "rp_mirror_polisher_stream_fasta": (_u32, [_vp, _int, _str, _str, _u64, _int, _int]),
+    "rp_mirror_polish_files_grouped": (_int, [_str, _str, _str, _int, _u32, C.c_double, C.c_double, _int, _i8, _i8, _i8,
+                                              _vp, _u32, _int, _u64, _int, _u64, _str, _vp, _vp, _u32]),
+    "rp_mirror_last_grouped_run": (None, [_vp, _vp, _vp, _vp]),
+    "rp_mirror_plan_read_groups": (C.c_int64, [_u64, _u32, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp,
+                                               _u32]),
     "rp_mirror_format_fasta": (_u64, [_str, _str, _str, _u64, _str, _u64]),
     "rp_mirror_stitch_order": (_u64, [_u32, _vp, _vp, _vp, _vp]),
     "rp_mirror_input_open": (_vp, [_str, _str, _str, _int, C.c_double, _vp, _u32]),
@@ -749,13 +755,79 @@ class InputFiles:
             pass
 
 
+def device_memory(device=0):
+    """(free bytes, total bytes) of a CUDA device (rp_device_memory)."""
+    lib = load()
+    free, total = C.c_uint64(), C.c_uint64()
+    _check(lib, lib.rp_device_memory(device, C.byref(free), C.byref(total)), "rp_device_memory")
+    return free.value, total.value
+
+
+def read_store_bytes(lengths, has_quality):
+    """What rp_reads_create allocates for sequences of these lengths (include/racon_b200.h, rp_reads_bytes)."""
+    lengths = np.asarray(lengths, dtype=np.uint64)
+    quality = bool(np.any((np.asarray(has_quality) != 0) & (lengths > 0)))
+    return (int(lengths.sum()) + 16) * (2 if quality else 1)
+
+
+def plan_read_groups(n_targets, lengths, has_quality, q_id, t_id, budget):
+    """The target groups the host layer polishes in under a read store budget of `budget` bytes per device (host only):
+    sequences of `lengths` (the first n_targets are the targets) with a quality string where has_quality, overlap k from
+    sequence q_id[k] onto target t_id[k].  Returns (first_target: group g = targets [first_target[g],
+    first_target[g + 1]), bytes: predicted store bytes per group, overlap_first, overlap_order: group g's overlaps are
+    overlap_order[overlap_first[g]:overlap_first[g + 1]]).  Raises RaconB200Error when one target does not fit."""
+    lib = load()
+    lengths = np.ascontiguousarray(lengths, dtype=np.uint32)
+    has_quality = np.ascontiguousarray(has_quality, dtype=np.uint8)
+    q_id = np.ascontiguousarray(q_id, dtype=np.uint32)
+    t_id = np.ascontiguousarray(t_id, dtype=np.uint32)
+    first = np.zeros(n_targets + 1, np.uint64)
+    nbytes = np.zeros(max(n_targets, 1), np.uint64)
+    ofirst = np.zeros(n_targets + 1, np.uint64)
+    order = np.zeros(max(len(q_id), 1), np.uint64)
+    err = C.create_string_buffer(1024)
+    n = lib.rp_mirror_plan_read_groups(n_targets, len(lengths), _ptr(lengths), _ptr(has_quality), len(q_id), _ptr(q_id),
+                                       _ptr(t_id), budget, _ptr(first), _ptr(nbytes), _ptr(ofirst), _ptr(order), err,
+                                       len(err))
+    if n < 0:
+        raise RaconB200Error(err.value.decode(errors="replace"))
+    return first[:n + 1], nbytes[:n], ofirst[:n + 1], order[:len(q_id)]
+
+
+def last_grouped_run():
+    """The last polish_files run of this process (with resident_reads): rp_reads_bytes of each target group's read store,
+    and the whole-run indices of the overlaps and windows the device refused."""
+    lib = load()
+    counts = np.zeros(3, np.uint64)
+    lib.rp_mirror_last_grouped_run(_ptr(counts), None, None, None)
+    out = [np.zeros(max(int(n), 1), np.uint64) for n in counts]
+    lib.rp_mirror_last_grouped_run(_ptr(counts), *[_ptr(a) for a in out])
+    return {k: [int(v) for v in a[:int(n)]]
+            for k, a, n in zip(("group_bytes", "failed_overlaps", "failed_windows"), out, counts)}
+
+
 def polish_files(reads, overlaps, targets, out_path, fragment_correction=False, window_length=500, quality_threshold=10.0,
                  error_threshold=0.3, trim=True, match=3, mismatch=-5, gap=-4, device=0, drop_unpolished=True,
-                 mem_bytes=0, banded=False, resident_reads=True):
+                 mem_bytes=0, banded=False, resident_reads=True, read_store_bytes=0):
     """racon's whole run through the C++ host layer: files in, polished FASTA out (alignment, breaking points and
     consensus on the device).  device: a CUDA device index or a sequence of them — device=range(device_count()) runs on
-    every visible GPU; the file is byte-identical whatever the list.  Returns (records written, overlaps the device
-    refused, windows the device refused)."""
+    every visible GPU; the file is byte-identical whatever the list.  With resident_reads (the default) the targets are
+    polished in consecutive groups whose sequences fit a device read store of read_store_bytes per device (0 = half of
+    the smallest free device memory); the file is the same whatever the groups.  Returns (records written, overlaps the
+    device refused, windows the device refused)."""
+    if resident_reads:
+        lib = load()
+        devices = _device_list(device)
+        err = C.create_string_buffer(1024)
+        result = np.zeros(3, np.uint64)
+        st = lib.rp_mirror_polish_files_grouped(
+            os.fsencode(reads), os.fsencode(overlaps), os.fsencode(targets), 1 if fragment_correction else 0,
+            window_length, quality_threshold, error_threshold, 1 if trim else 0, match, mismatch, gap, _ptr(devices),
+            len(devices), 1 if drop_unpolished else 0, mem_bytes, 1 if banded else 0, read_store_bytes,
+            os.fsencode(out_path), _ptr(result), err, len(err))
+        if st != 0:
+            raise RaconB200Error(err.value.decode(errors="replace"))
+        return tuple(int(v) for v in result)
     pol = MirrorPolisher.from_files(reads, overlaps, targets, fragment_correction=fragment_correction,
                                     window_length=window_length, quality_threshold=quality_threshold,
                                     error_threshold=error_threshold, trim=trim, match=match, mismatch=mismatch, gap=gap,

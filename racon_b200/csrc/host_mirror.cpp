@@ -352,6 +352,7 @@ const rp_reads* Polisher::read_store(uint32_t device) {
     std::vector<const char*> data(sequences_.size()), quality(sequences_.size());
     std::vector<uint32_t> length(sequences_.size());
     for (size_t i = 0; i < sequences_.size(); ++i) {
+        if (!store_members_.empty() && !store_members_[i]) continue;   // absent: length 0, no bytes on the device
         data[i] = sequences_[i].data;
         quality[i] = sequences_[i].quality;
         length[i] = sequences_[i].length;
@@ -479,7 +480,8 @@ void Polisher::align(std::vector<Overlap>& overlaps, const std::vector<size_t>& 
             if (st != RP_ALN_OK) {
                 /* the reference re-aligns such overlaps with its CPU edlib (cudapolisher.cpp:213); this path has no CPU
                  * aligner, so the overlap contributes no layers and the caller is told */
-                fprintf(stderr, "[racon_b200::Polisher] warning: overlap %zu exceeded device limit %u\n", k, st);
+                fprintf(stderr, "[racon_b200::Polisher] warning: overlap %zu exceeded device limit %u\n",
+                        static_cast<size_t>(overlap_ids_ ? overlap_ids_[k] : k), st);
                 failed_overlaps_.push_back(k);
                 continue;
             }
@@ -498,11 +500,13 @@ void Polisher::initialize(std::vector<Overlap>& overlaps) {
     build_windows(overlaps);
 }
 
-void Polisher::build_windows(const std::vector<Overlap>& overlaps) {
+void Polisher::build_windows(const std::vector<Overlap>& overlaps) { build_windows(overlaps, 0, targets_size_); }
 
-    /* one window per window_length_ bases of every target (polisher.cpp:383-401) */
-    std::vector<uint64_t> id_to_first_window_id(targets_size_ + 1, 0);
-    for (uint64_t i = 0; i < targets_size_; ++i) {
+void Polisher::build_windows(const std::vector<Overlap>& overlaps, uint64_t first_target, uint64_t end_target) {
+
+    /* one window per window_length_ bases of every target (polisher.cpp:383-401), appended to windows_ */
+    std::vector<uint64_t> id_to_first_window_id(end_target - first_target + 1, windows_.size());
+    for (uint64_t i = first_target; i < end_target; ++i) {
         uint32_t k = 0;
         const SequenceView& tgt = sequences_[i];
         for (uint32_t j = 0; j < tgt.length; j += window_length_, ++k) {
@@ -511,10 +515,11 @@ void Polisher::build_windows(const std::vector<Overlap>& overlaps) {
                                                tgt.quality ? tgt.quality + j : dummy_quality_.data(), length));
             windows_.back()->set_backbone_origin(static_cast<uint32_t>(i), j);
         }
-        id_to_first_window_id[i + 1] = id_to_first_window_id[i] + k;
+        id_to_first_window_id[i - first_target + 1] = id_to_first_window_id[i - first_target] + k;
     }
 
-    targets_coverages_.assign(targets_size_, 0);
+    targets_coverages_.resize(targets_size_);
+    std::fill(targets_coverages_.begin() + first_target, targets_coverages_.begin() + end_target, 0);
 
     /* one layer per pair of breaking points (polisher.cpp:405-458) */
     for (uint64_t i = 0; i < overlaps.size(); ++i) {
@@ -535,7 +540,8 @@ void Polisher::build_windows(const std::vector<Overlap>& overlaps) {
                 if (average_quality < quality_threshold_) continue;
             }
 
-            const uint64_t window_id = id_to_first_window_id[o.t_id] + breaking_points[j].first / window_length_;
+            const uint64_t window_id =
+                id_to_first_window_id[o.t_id - first_target] + breaking_points[j].first / window_length_;
             const uint32_t window_start = (breaking_points[j].first / window_length_) * window_length_;
             const char* data = (o.strand ? reverse_complement(o.q_id) : sequence.data) + breaking_points[j].second;
             const uint32_t data_length = breaking_points[j + 1].second - breaking_points[j].second;
@@ -629,6 +635,154 @@ void Polisher::consensus_lanes(const std::function<void(const PolishedSequence&)
         stitcher.finish(slot.first, slot.count, stitch);
     };
     run_lanes(slots.size(), fill, ready, drain);
+}
+
+/* ---- target groups ---- */
+uint64_t read_store_bytes(uint64_t sum_of_lengths, bool any_quality) {
+    return (sum_of_lengths + 16) * (any_quality ? 2 : 1);
+}
+
+namespace {
+std::string over_budget(const std::string& target_name, uint64_t bytes, uint64_t budget) {
+    return "[racon_b200::Polisher] error: target " + target_name + " needs a read store of " + std::to_string(bytes) +
+           " bytes, over the budget of " + std::to_string(budget) + " bytes per device!";
+}
+}  // namespace
+
+TargetOverBudget::TargetOverBudget(uint64_t target, uint64_t bytes, uint64_t budget)
+    : std::runtime_error(over_budget("#" + std::to_string(target), bytes, budget)), target(target), bytes(bytes),
+      budget(budget) {}
+
+std::string TargetOverBudget::message(const std::string& target_name) const {
+    return over_budget(target_name, bytes, budget);
+}
+
+ReadGroups plan_read_groups(uint64_t targets_size, const std::vector<SequenceView>& sequences,
+                            const std::vector<Overlap>& overlaps, uint64_t budget) {
+    /* the overlaps of every target, in their original order (stable counting sort by t_id) */
+    std::vector<uint64_t> by_target_first(targets_size + 1, 0), by_target(overlaps.size());
+    for (const Overlap& o : overlaps) ++by_target_first[o.t_id + 1];
+    for (uint64_t t = 0; t < targets_size; ++t) by_target_first[t + 1] += by_target_first[t];
+    {
+        std::vector<uint64_t> at(by_target_first.begin(), by_target_first.end() - 1);
+        for (uint64_t k = 0; k < overlaps.size(); ++k) by_target[at[overlaps[k].t_id]++] = k;
+    }
+
+    ReadGroups g;
+    /* the open group's store: its sequences (member_of[i] == group index + 1), their summed length, any quality */
+    std::vector<uint64_t> member_of(sequences.size(), 0);
+    uint64_t sum = 0;
+    bool any_quality = false;
+    std::vector<uint32_t> fresh;   // the sequences target t adds to a group
+    uint64_t next_sum = 0;
+    bool next_quality = false;
+    /* the store bytes of group `stamp` - 1 (of `base_sum` / `base_quality` so far) with target t in it */
+    auto with_target = [&](uint64_t t, uint64_t stamp, uint64_t base_sum, bool base_quality) {
+        fresh.clear();
+        auto add = [&](uint32_t id) {
+            if (member_of[id] == stamp) return;
+            member_of[id] = stamp;
+            fresh.push_back(id);
+        };
+        add(static_cast<uint32_t>(t));
+        for (uint64_t k = by_target_first[t]; k < by_target_first[t + 1]; ++k) add(overlaps[by_target[k]].q_id);
+        next_sum = base_sum;
+        next_quality = base_quality;
+        for (uint32_t id : fresh) {
+            next_sum += sequences[id].length;
+            next_quality = next_quality || (sequences[id].quality != nullptr && sequences[id].length > 0);
+        }
+        return read_store_bytes(next_sum, next_quality);
+    };
+    for (uint64_t t = 0; t < targets_size; ++t) {
+        const bool open = g.size() > 0;
+        uint64_t bytes = open ? with_target(t, g.size(), sum, any_quality) : 0;
+        if (!open || bytes > budget) {   // t starts a group of its own
+            for (uint32_t id : fresh) member_of[id] = 0;
+            bytes = with_target(t, g.size() + 1, 0, false);
+            if (bytes > budget) throw TargetOverBudget(t, bytes, budget);
+            g.first_target.push_back(t);
+            g.bytes.push_back(0);
+        }
+        g.bytes.back() = bytes;
+        sum = next_sum;
+        any_quality = next_quality;
+    }
+    g.first_target.push_back(targets_size);
+
+    /* each group's overlaps in their original order (stable counting sort by group) */
+    std::vector<uint64_t> group_of(targets_size);
+    for (size_t k = 0; k < g.size(); ++k)
+        std::fill(group_of.begin() + g.first_target[k], group_of.begin() + g.first_target[k + 1], k);
+    g.overlap_first.assign(g.size() + 1, 0);
+    for (const Overlap& o : overlaps) ++g.overlap_first[group_of[o.t_id] + 1];
+    for (size_t k = 0; k < g.size(); ++k) g.overlap_first[k + 1] += g.overlap_first[k];
+    g.overlap_order.resize(overlaps.size());
+    std::vector<uint64_t> at(g.overlap_first.begin(), g.overlap_first.end() - 1);
+    for (uint64_t k = 0; k < overlaps.size(); ++k) g.overlap_order[at[group_of[overlaps[k].t_id]]++] = k;
+    return g;
+}
+
+void Polisher::polish_groups(std::vector<Overlap>& overlaps, const std::function<void(const PolishedSequence&)>& sink,
+                             bool drop_unpolished_sequences, size_t memory, bool banded, uint64_t read_store_bytes) {
+    std::vector<uint32_t> distinct;
+    for (uint32_t d : devices_)
+        if (std::find(distinct.begin(), distinct.end(), d) == distinct.end()) distinct.push_back(d);
+    if (read_store_bytes == 0) {   // half of the smallest free memory, before any store or batch object exists
+        uint64_t smallest = ~0ull;
+        for (uint32_t d : distinct) {
+            uint64_t free_b = 0, total_b = 0;
+            const rp_status s = rp_device_memory(static_cast<int>(d), &free_b, &total_b);
+            if (s != RP_OK) hard_error("[racon_b200::Polisher::polish_groups] error: " + status_text(s));
+            smallest = std::min(smallest, free_b);
+        }
+        read_store_bytes = smallest / 2;
+    }
+    const ReadGroups groups = plan_read_groups(targets_size_, sequences_, overlaps, read_store_bytes);
+
+    resident_reads_ = true;
+    group_store_bytes_.clear();
+    std::vector<size_t> failed_overlaps, failed_windows;   // whole-run indices
+    uint64_t windows_before = 0;                           // windows of the groups before this one
+    for (size_t g = 0; g < groups.size(); ++g) {
+        const uint64_t first = groups.first_target[g], end = groups.first_target[g + 1];
+        /* the group's overlaps, in their original order, moved out and back */
+        std::vector<Overlap> subset;
+        subset.reserve(groups.overlap_first[g + 1] - groups.overlap_first[g]);
+        for (uint64_t k = groups.overlap_first[g]; k < groups.overlap_first[g + 1]; ++k)
+            subset.push_back(std::move(overlaps[groups.overlap_order[k]]));
+        auto global_overlap = [&](size_t local) { return groups.overlap_order[groups.overlap_first[g] + local]; };
+
+        /* the store first, on every distinct device: the batch objects then size themselves from what is left */
+        store_members_.assign(sequences_.size(), 0);
+        std::fill(store_members_.begin() + first, store_members_.begin() + end, 1);
+        for (const Overlap& o : subset) store_members_[o.q_id] = 1;
+        run_stage([&] {
+            for (uint32_t d : distinct) read_store(d);
+        }, [&] { release_read_stores(); });
+        group_store_bytes_.push_back(rp_reads_bytes(stores_.front().second));
+
+        failed_overlaps_.clear();
+        overlap_ids_ = groups.overlap_order.data() + groups.overlap_first[g];   // warnings name whole-run indices
+        find_overlap_breaking_points(subset);
+        overlap_ids_ = nullptr;
+        for (size_t k : failed_overlaps_) failed_overlaps.push_back(global_overlap(k));
+
+        windows_.clear();
+        build_windows(subset, first, end);
+        failed_windows_.clear();
+        consensus(sink, drop_unpolished_sequences, memory, banded, true, true);
+        for (size_t w : failed_windows_) failed_windows.push_back(windows_before + w);
+        windows_before += windows_.size();
+
+        release_read_stores();
+        for (uint64_t k = 0; k < subset.size(); ++k) overlaps[global_overlap(k)] = std::move(subset[k]);
+    }
+    store_members_.clear();
+    windows_.clear();
+    std::sort(failed_overlaps.begin(), failed_overlaps.end());
+    failed_overlaps_ = std::move(failed_overlaps);
+    failed_windows_ = std::move(failed_windows);   // groups in target order: already sorted
 }
 
 }  // namespace racon_b200
@@ -846,6 +1000,110 @@ extern "C" uint32_t rp_mirror_polisher_stream_fasta(void* hv, int drop_unpolishe
 }
 
 extern "C" void rp_mirror_polisher_close(void* hv) { delete static_cast<PolHandle*>(hv); }
+
+namespace {
+/* the last rp_mirror_polish_files_grouped (rp_mirror_last_grouped_run) */
+std::vector<uint64_t> g_last_group_store_bytes, g_last_failed_overlaps, g_last_failed_windows;
+}  // namespace
+
+/* racon's whole run on files in target groups (Polisher::polish_groups): load_input, plan, polish, FASTA into `path`.
+ * read_store_bytes: budget per device (0 = automatic).  result[0] = records written, [1] overlaps and [2] windows the
+ * device refused.  Returns 0, or -1 with the message in err (input error, a target over the budget, unwritable path). */
+extern "C" int rp_mirror_polish_files_grouped(const char* reads, const char* overlaps, const char* targets,
+                                              int fragment_correction, uint32_t window_length, double quality_threshold,
+                                              double error_threshold, int trim, int8_t match, int8_t mismatch, int8_t gap,
+                                              const uint32_t* devices, uint32_t n_devices, int drop_unpolished,
+                                              uint64_t mem_bytes, int banded, uint64_t read_store_bytes,
+                                              const char* path, uint64_t* result, char* err, uint32_t err_cap) {
+    using namespace racon_b200;
+    auto error = [&](const std::string& what) {
+        if (err && err_cap) {
+            std::strncpy(err, what.c_str(), err_cap - 1);
+            err[err_cap - 1] = '\0';
+        }
+        return -1;
+    };
+    InputSet input;
+    try {
+        input = load_input(reads, overlaps, targets, fragment_correction != 0, error_threshold);
+    } catch (const std::exception& e) {
+        return error(e.what());
+    }
+    Polisher polisher(input.views(), input.targets_size, input.window_type, fragment_correction != 0, window_length,
+                      quality_threshold, trim != 0, match, mismatch, gap,
+                      std::vector<uint32_t>(devices, devices + n_devices));
+    FILE* f = std::fopen(path, "wb");
+    if (!f) return error(std::string("cannot write ") + path);
+    uint64_t n = 0;
+    try {
+        polisher.polish_groups(input.overlaps,
+                               [&](const PolishedSequence& s) {
+                                   const std::string rec = format_fasta(input.sequences[s.id].name, s);
+                                   std::fwrite(rec.data(), 1, rec.size(), f);
+                                   ++n;
+                               },
+                               drop_unpolished != 0, static_cast<size_t>(mem_bytes), banded != 0, read_store_bytes);
+    } catch (const TargetOverBudget& e) {   // planned before any record: no output
+        std::fclose(f);
+        std::remove(path);
+        return error(e.message(input.sequences[e.target].name));
+    }
+    std::fclose(f);
+    g_last_group_store_bytes = polisher.group_store_bytes();
+    g_last_failed_overlaps.assign(polisher.failed_overlaps().begin(), polisher.failed_overlaps().end());
+    g_last_failed_windows.assign(polisher.failed_windows().begin(), polisher.failed_windows().end());
+    result[0] = n;
+    result[1] = polisher.failed_overlaps().size();
+    result[2] = polisher.failed_windows().size();
+    return 0;
+}
+
+/* The last rp_mirror_polish_files_grouped: counts[0] groups, [1] failed overlaps, [2] failed windows; then (any pointer
+ * may be NULL) rp_reads_bytes of every group's store and the whole-run indices of the failed overlaps and windows. */
+extern "C" void rp_mirror_last_grouped_run(uint64_t* counts, uint64_t* group_bytes, uint64_t* failed_overlaps,
+                                           uint64_t* failed_windows) {
+    counts[0] = g_last_group_store_bytes.size();
+    counts[1] = g_last_failed_overlaps.size();
+    counts[2] = g_last_failed_windows.size();
+    if (group_bytes) std::copy(g_last_group_store_bytes.begin(), g_last_group_store_bytes.end(), group_bytes);
+    if (failed_overlaps) std::copy(g_last_failed_overlaps.begin(), g_last_failed_overlaps.end(), failed_overlaps);
+    if (failed_windows) std::copy(g_last_failed_windows.begin(), g_last_failed_windows.end(), failed_windows);
+}
+
+/* Host-only hook of plan_read_groups: n_seq sequences (the first n_targets are the targets) of length[i], with a quality
+ * string when has_quality[i]; overlap k runs from sequence q_id[k] onto target t_id[k].  Outputs (capacities: n_targets + 1
+ * groups at most): group g = targets [first_target[g], first_target[g + 1]), predicted store bytes[g], and its overlaps
+ * overlap_order[overlap_first[g] .. overlap_first[g + 1]) (n_overlaps entries in all).  Returns the number of groups, or
+ * -1 with the error in err (a target over the budget). */
+extern "C" int64_t rp_mirror_plan_read_groups(uint64_t n_targets, uint32_t n_seq, const uint32_t* length,
+                                              const uint8_t* has_quality, uint64_t n_overlaps, const uint32_t* q_id,
+                                              const uint32_t* t_id, uint64_t budget, uint64_t* first_target,
+                                              uint64_t* bytes, uint64_t* overlap_first, uint64_t* overlap_order,
+                                              char* err, uint32_t err_cap) {
+    using namespace racon_b200;
+    static const char kQuality[] = "";   // stands for "has a quality string": the planner only tests for null
+    std::vector<SequenceView> seqs(n_seq);
+    for (uint32_t i = 0; i < n_seq; ++i) seqs[i] = SequenceView{nullptr, has_quality[i] ? kQuality : nullptr, length[i]};
+    std::vector<Overlap> ovl(n_overlaps);
+    for (uint64_t k = 0; k < n_overlaps; ++k) {
+        ovl[k].q_id = q_id[k];
+        ovl[k].t_id = t_id[k];
+    }
+    try {
+        const ReadGroups g = plan_read_groups(n_targets, seqs, ovl, budget);
+        std::copy(g.first_target.begin(), g.first_target.end(), first_target);
+        std::copy(g.bytes.begin(), g.bytes.end(), bytes);
+        std::copy(g.overlap_first.begin(), g.overlap_first.end(), overlap_first);
+        std::copy(g.overlap_order.begin(), g.overlap_order.end(), overlap_order);
+        return static_cast<int64_t>(g.size());
+    } catch (const std::exception& e) {
+        if (err && err_cap) {
+            std::strncpy(err, e.what(), err_cap - 1);
+            err[err_cap - 1] = '\0';
+        }
+        return -1;
+    }
+}
 
 /* Host-only test hook of the stitch cursor (InOrderStitcher): n_ranges contiguous ranges of counts[r] windows finish in
  * the order `completion` (a permutation of 0 .. n_ranges - 1).  order[i] = the i-th window emitted, step[i] = the position

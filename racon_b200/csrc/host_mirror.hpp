@@ -11,6 +11,7 @@
 #include <atomic>
 #include <functional>
 #include <memory>
+#include <stdexcept>
 #include <string>
 #include <utility>
 #include <vector>
@@ -217,6 +218,35 @@ private:
     size_t cursor_ = 0;
 };
 
+/* ---- target groups: polishing a read set larger than one device's memory -------------------------------------------
+ * A group is a contiguous range of targets together with the read store of exactly the sequences it needs: its targets
+ * and every read with an overlap onto one of them.  Its store costs read_store_bytes() of those sequences
+ * (rp_reads_bytes' rule).  A read needed by two groups (racon -f, reads spanning contig ends) is counted in both. */
+uint64_t read_store_bytes(uint64_t sum_of_lengths, bool any_quality);
+
+struct ReadGroups {
+    std::vector<uint64_t> first_target;    // group g = targets [first_target[g], first_target[g + 1])
+    std::vector<uint64_t> bytes;           // predicted rp_reads_bytes of group g's store
+    /* group g's overlaps, as indices into the overlaps, in their original (file) order: a window's layer order is the
+     * order of its overlaps, and it decides the consensus */
+    std::vector<uint64_t> overlap_first;   // group g = overlap_order[overlap_first[g] .. overlap_first[g + 1])
+    std::vector<uint64_t> overlap_order;
+    size_t size() const { return bytes.size(); }
+};
+
+/* A single target whose own store exceeds the budget: it cannot be polished under that budget. */
+struct TargetOverBudget : std::runtime_error {
+    uint64_t target, bytes, budget;
+    TargetOverBudget(uint64_t target, uint64_t bytes, uint64_t budget);
+    std::string message(const std::string& target_name) const;
+};
+
+/* Greedy over the targets in order: a group is closed when its next target would push its store over `budget` bytes.
+ * Host only.  Reads sequences[i].length and whether sequences[i].quality is set, and t_id / q_id of every overlap.
+ * Throws TargetOverBudget. */
+ReadGroups plan_read_groups(uint64_t targets_size, const std::vector<SequenceView>& sequences,
+                            const std::vector<Overlap>& overlaps, uint64_t budget);
+
 /* The polisher runs its two device stages on a list of devices: one lane per entry (the same device may appear more than
  * once: {0, 0} = two lanes on one GPU).  The aligner has one batch object per lane, the consensus two; one host thread
  * hands every idle object the next contiguous range of overlaps / windows, launches it asynchronously and collects
@@ -241,6 +271,8 @@ public:
     void initialize(std::vector<Overlap>& overlaps);
     /* the window-building half of initialize() alone, for overlaps whose breaking points are already known */
     void build_windows(const std::vector<Overlap>& overlaps);
+    /* the same for targets [first_target, end_target) alone, whose overlaps those are */
+    void build_windows(const std::vector<Overlap>& overlaps, uint64_t first_target, uint64_t end_target);
     void polish(std::vector<PolishedSequence>& dst, bool drop_unpolished_sequences);
     /* Streaming form (polisher.cpp:504-537 + main.cpp:159-161 as a consumer overlapped with the compute): two batch
      * objects per lane stay in flight; while they run on the GPUs the finished windows are stitched in window order, and
@@ -250,6 +282,16 @@ public:
      * once (rp_reads) and add the windows by reference — layer extraction on the device, no host copy of layer bytes. */
     void polish_streaming(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
                           size_t memory = 0, bool banded = false, bool resident_reads = false);
+    /* initialize + polish_streaming(resident_reads = true) in target groups (plan_read_groups): for each group in target
+     * order, its store goes to every distinct device, its overlaps are aligned, its windows built and polished, its records
+     * streamed to `sink`, and its store released.  `read_store_bytes` = budget per device (0 = half of the smallest free
+     * memory of the devices, read before anything is allocated).  The overlaps come from load_input (filter and window
+     * type over the whole input); failed_overlaps / failed_windows keep their whole-run indices.  With one group the
+     * output is that of initialize + polish_streaming.  Throws TargetOverBudget before any device work. */
+    void polish_groups(std::vector<Overlap>& overlaps, const std::function<void(const PolishedSequence&)>& sink,
+                       bool drop_unpolished_sequences, size_t memory, bool banded, uint64_t read_store_bytes);
+    /* rp_reads_bytes of each group's store in the last polish_groups (of the first device's copy) */
+    const std::vector<uint64_t>& group_store_bytes() const { return group_store_bytes_; }
     const std::vector<std::shared_ptr<Window>>& windows() const { return windows_; }
     /* Items the device could not finish (soft RP_ALN_* / RP_WIN_* status).  The reference hands such items to its CPU
      * code (cudapolisher.cpp:213 edlib, :354-370 spoa); this library has no CPU path, so a failed overlap contributes
@@ -290,6 +332,9 @@ private:
     std::vector<size_t> failed_overlaps_, failed_windows_;
     bool resident_reads_ = false;
     std::vector<std::pair<uint32_t, rp_reads*>> stores_;   // (device, store): one per distinct device, made at first use
+    std::vector<uint8_t> store_members_;   // empty: stores hold every sequence; else those i with store_members_[i]
+    std::vector<uint64_t> group_store_bytes_;
+    const uint64_t* overlap_ids_ = nullptr;   // while a group is aligned: whole-run index of each overlap of the group
     const rp_reads* read_store(uint32_t device);
 };
 

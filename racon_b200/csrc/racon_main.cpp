@@ -6,10 +6,11 @@
  * The option table and its parsing are racon 1.5.0's with CUDA support (getopt_long over "ufw:q:e:m:x:g:t:hbc::", atoi /
  * atof conversions, int8_t scores, `-c` taking its count from the next word when that word is not an option).  The run is
  * the host layer's: load_input (parsing + racon's overlap filter), then Polisher on every visible GPU (alignment,
- * breaking points and consensus on the device) and polish_streaming, whose sink writes each record to stdout the moment
- * it is stitched.
+ * breaking points and consensus on the device) in target groups whose sequences fit the device read store budget
+ * (polish_groups, RP_READ_STORE_BYTES), whose sink writes each record to stdout the moment it is stitched.
  *
- * Exit status: 0 = racon's bytes; 1 = an error (bad argument, bad input, no device, a device error, a failed write);
+ * Exit status: 0 = racon's bytes; 1 = an error (bad argument, bad input, no device, a target over the read store budget, a device error,
+ * a failed write);
  * 2 = the output was written, but the device refused some overlaps or windows (a soft RP_ALN_* / RP_WIN_* status).  racon
  * redoes such items on its CPU; this program has no CPU path, so its output then differs from racon's.
  */
@@ -87,9 +88,31 @@ void usage(FILE* out) {
         "    --cudaaligner-batches <int>    alignment always runs on the device; the lanes decide the batches\n"
         "    --cudaaligner-band-width <int> alignment is always exact (edlib's result)\n"
         "\n"
+        "environment:\n"
+        "    RP_READ_STORE_BYTES=<bytes>    device memory per GPU for the sequences of one group of targets: the targets\n"
+        "                                   are polished in consecutive groups whose sequences fit it, with the output of\n"
+        "                                   one pass.  Unset or 0: half of the smallest free GPU memory.  A target whose\n"
+        "                                   own sequences do not fit is an error (status 1)\n"
+        "\n"
         "exit status: 0 = output written; 1 = error; 2 = output written, but the device refused some overlaps or\n"
         "windows, which racon would have redone on its CPU: the output then differs from racon's.\n",
         out);
+}
+
+/* RP_READ_STORE_BYTES: the read store budget per device, in bytes (unset, empty or 0 = automatic: half of the smallest
+ * free device memory).  false when it is not a plain decimal number that fits 64 bits. */
+bool read_store_budget(uint64_t* bytes) {
+    *bytes = 0;
+    const char* s = getenv("RP_READ_STORE_BYTES");
+    if (s == nullptr || *s == '\0') return true;
+    for (const char* c = s; *c; ++c) {
+        if (*c < '0' || *c > '9') return false;
+    }
+    errno = 0;
+    const unsigned long long v = strtoull(s, nullptr, 10);
+    if (errno == ERANGE) return false;
+    *bytes = v;
+    return true;
 }
 
 /* thrown by the output sink: unwinds through the polisher, whose batch objects and read stores are released on the way */
@@ -151,6 +174,12 @@ int main(int argc, char** argv) {
         fprintf(stderr, "[racon_b200::main] error: invalid window length!\n");
         return 1;
     }
+    uint64_t read_store_bytes = 0;
+    if (!read_store_budget(&read_store_bytes)) {
+        fprintf(stderr, "[racon_b200::main] error: RP_READ_STORE_BYTES must be a decimal byte count, not \"%s\"!\n",
+                getenv("RP_READ_STORE_BYTES"));
+        return 1;
+    }
     racon_b200::InputSet input;
     try {
         input = racon_b200::load_input(reads_path, overlaps_path, targets_path, fragment_correction, error_threshold);
@@ -179,18 +208,20 @@ int main(int argc, char** argv) {
     try {
         racon_b200::Polisher polisher(input.views(), input.targets_size, input.window_type, fragment_correction,
                                       window_length, quality_threshold, trim, match, mismatch, gap, devices);
-        polisher.use_resident_reads(true);
-        polisher.initialize(input.overlaps);
-        polisher.polish_streaming(
+        polisher.polish_groups(
+            input.overlaps,
             [&](const racon_b200::PolishedSequence& s) {
                 const std::string record = racon_b200::format_fasta(input.sequences[s.id].name, s);
                 if (fwrite(record.data(), 1, record.size(), stdout) != record.size()) throw WriteError(errno);
             },
-            drop_unpolished_sequences, 0, banded, true);
+            drop_unpolished_sequences, 0, banded, read_store_bytes);
         failed_overlaps = polisher.failed_overlaps().size();
         failed_windows = polisher.failed_windows().size();
     } catch (const WriteError& e) {
         fprintf(stderr, "[racon_b200::main] error: writing the output failed: %s\n", strerror(e.error));
+        return 1;
+    } catch (const racon_b200::TargetOverBudget& e) {
+        fprintf(stderr, "%s\n", e.message(input.sequences[e.target].name).c_str());
         return 1;
     }
     if (fflush(stdout) != 0 || ferror(stdout)) {

@@ -77,6 +77,13 @@ struct DevBuf {
         cap = e == cudaSuccess ? nc : 0;
         return e;
     }
+    /* exactly n bytes, no head room: for buffers that never grow (the read store, whose size callers plan with) */
+    cudaError_t allocate_exact(size_t n) {
+        release();
+        cudaError_t e = cudaMalloc(&p, n);
+        cap = e == cudaSuccess ? n : 0;
+        return e;
+    }
     void release() {
         if (p) cudaFree(p);
         p = nullptr;
@@ -444,6 +451,17 @@ int rp_device_count(void) {
     return n;
 }
 
+rp_status rp_device_memory(int device, uint64_t* free_bytes, uint64_t* total_bytes) {
+    if (!free_bytes || !total_bytes) return fail(RP_ERR_INVALID, "null argument");
+    const rp_status s = check_device(device);
+    if (s != RP_OK) return s;
+    size_t free_b = 0, total_b = 0;
+    RP_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    *free_bytes = free_b;
+    *total_bytes = total_b;
+    return RP_OK;
+}
+
 rp_status rp_poa_create(rp_poa** out, int device, size_t mem_bytes, int8_t match, int8_t mismatch, int8_t gap,
                         int banded, uint32_t window_len_hint, uint32_t max_depth_hint) {
     (void)max_depth_hint;
@@ -657,8 +675,9 @@ rp_status rp_reads_create(rp_reads** out, int device, uint32_t n_seqs, const cha
             if (seen[c]) r->chars[i][c >> 6] |= 1ull << (c & 63);
     }
     const uint64_t total = r->off[n_seqs];
-    cudaError_t e = r->d_bases.reserve(total + 16);
-    if (e == cudaSuccess && r->any_quality) e = r->d_quals.reserve(total + 16);
+    /* the size rule of racon_b200.h (rp_reads_bytes): callers plan their read stores with it */
+    cudaError_t e = r->d_bases.allocate_exact(total + 16);
+    if (e == cudaSuccess && r->any_quality) e = r->d_quals.allocate_exact(total + 16);
     /* the caller's sequences are separate pageable strings: stage them through pinned memory in large pieces */
     const size_t stage_bytes = static_cast<size_t>(std::min<uint64_t>(std::max<uint64_t>(total, 1), 64ull << 20));
     void* stage = nullptr;

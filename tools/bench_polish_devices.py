@@ -12,7 +12,12 @@ total_s, which is one parse + the device stages, as in polish_files), overlaps (
 per second, speedup and scaling efficiency against [0] from total_s, the CPU time of the driving thread, the md5 of the
 FASTA (the same in every row), and the card's name and power limit.
 
-  python tools/bench_polish_devices.py [--genome-mb 16] [--coverage 30] [--seed 1]
+With --read-store-bytes B: on device [0] only, api.polish_files in target groups, alternating runs under the automatic
+budget (one group here) and under B bytes per device, three of each.  One JSON line per run: the load alone, the whole
+grouped run (parse, plan, and per group: store upload, alignment, window building, consensus + FASTA), the groups and their
+store bytes, the md5 of the FASTA.
+
+  python tools/bench_polish_devices.py [--genome-mb 16] [--coverage 30] [--seed 1] [--read-store-bytes B]
 """
 import argparse
 import ctypes
@@ -139,6 +144,20 @@ def polish(d, devices, out):
                 md5=hashlib.md5(open(out, "rb").read()).hexdigest())
 
 
+def polish_grouped(d, budget, out):
+    """api.polish_files(read_store_bytes=budget) on device [0], timed; the load alone is timed beforehand"""
+    files = [os.path.join(d, f) for f in ("reads.fastq", "overlaps.paf", "reads.fastq")]
+    t0 = time.perf_counter()
+    api.InputFiles(*files, fragment_correction=True).close()
+    t1 = time.perf_counter()
+    n, fo, fw = api.polish_files(*files, out, fragment_correction=True, device=[0], read_store_bytes=budget)
+    t2 = time.perf_counter()
+    groups = api.last_grouped_run()["group_bytes"]
+    return dict(read_store_bytes=budget, load_s=round(t1 - t0, 3), grouped_total_s=round(t2 - t1, 3),
+                groups=len(groups), group_store_bytes=groups, records=n, failed=[fo, fw],
+                md5=hashlib.md5(open(out, "rb").read()).hexdigest())
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--genome-mb", type=float, default=16.0)
@@ -146,6 +165,8 @@ def main():
     ap.add_argument("--read-len", type=int, default=10000)
     ap.add_argument("--min-overlap", type=int, default=1000)
     ap.add_argument("--seed", type=int, default=1)
+    ap.add_argument("--read-store-bytes", type=int, default=None,
+                    help="compare target groups under this budget with the automatic budget, on device [0]")
     args = ap.parse_args()
     n_gpus = api.device_count()
     if n_gpus < 1:
@@ -160,6 +181,11 @@ def main():
         os.makedirs(warm)
         make_workload(warm, 0.2, 10, 5000, 1000, args.seed + 1)     # CUDA contexts and modules on every device
         polish(warm, sorted(set(sum(runs, []))), os.path.join(warm, "o.fasta"))
+        if args.read_store_bytes is not None:
+            for budget in (0, args.read_store_bytes) * 3:
+                row = dict(workload=size, cards=gpus[:1], **polish_grouped(d, budget, os.path.join(d, "polished.fasta")))
+                print(json.dumps(row), flush=True)
+            return
         base = None
         for devices in runs:
             r = polish(d, devices, os.path.join(d, "polished.fasta"))
