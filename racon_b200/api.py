@@ -95,10 +95,13 @@ HOST_SIGNATURES = {
     "rp_mirror_polisher_breaking_points": (_u64, [_vp, _vp, _vp]),
     "rp_mirror_polisher_stream_fasta": (_u32, [_vp, _int, _str, _str, _u64, _int, _int]),
     "rp_mirror_polish_files_grouped": (_int, [_str, _str, _str, _int, _u32, C.c_double, C.c_double, _int, _i8, _i8, _i8,
-                                              _vp, _u32, _int, _u64, _int, _u64, _str, _vp, _vp, _u32]),
+                                              _vp, _u32, _int, _u64, _int, _u64, _int, _str, _vp, _vp, _u32]),
     "rp_mirror_last_grouped_run": (None, [_vp, _vp, _vp, _vp]),
+    "rp_mirror_last_grouped_run_windows": (None, [_vp, _vp]),
     "rp_mirror_plan_read_groups": (C.c_int64, [_u64, _u32, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp,
                                                _u32]),
+    "rp_mirror_plan_split_read_groups": (C.c_int64, [_u64, _u32, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _u32, _u64, _vp,
+                                                     _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32]),
     "rp_mirror_format_fasta": (_u64, [_str, _str, _str, _u64, _str, _u64]),
     "rp_mirror_stitch_order": (_u64, [_u32, _vp, _vp, _vp, _vp]),
     "rp_mirror_input_open": (_vp, [_str, _str, _str, _int, C.c_double, _vp, _u32]),
@@ -770,22 +773,48 @@ def read_store_bytes(lengths, has_quality):
     return (int(lengths.sum()) + 16) * (2 if quality else 1)
 
 
-def plan_read_groups(n_targets, lengths, has_quality, q_id, t_id, budget):
+def plan_read_groups(n_targets, lengths, has_quality, q_id, t_id, budget, *, t_begin=None, t_end=None,
+                     window_length=None):
     """The target groups the host layer polishes in under a read store budget of `budget` bytes per device (host only):
     sequences of `lengths` (the first n_targets are the targets) with a quality string where has_quality, overlap k from
     sequence q_id[k] onto target t_id[k].  Returns (first_target: group g = targets [first_target[g],
     first_target[g + 1]), bytes: predicted store bytes per group, overlap_first, overlap_order: group g's overlaps are
-    overlap_order[overlap_first[g]:overlap_first[g + 1]]).  Raises RaconB200Error when one target does not fit."""
+    overlap_order[overlap_first[g]:overlap_first[g + 1]]).  Raises RaconB200Error when one target does not fit.
+
+    With window_length (and every overlap's target span [t_begin[k], t_end[k])) a target that does not fit is split
+    into parts of consecutive windows, as polish_files(split_targets=True) polishes it.  The result then also carries
+    first_window, end_window (group g is windows [first_window[g], end_window[g]) of its one target when it is a part;
+    0, 0 for a group of whole targets) and aligned_in (the group that aligns overlap k: the first it is in); an overlap
+    is in every part it touches.  Raises RaconB200Error when one window does not fit."""
     lib = load()
     lengths = np.ascontiguousarray(lengths, dtype=np.uint32)
     has_quality = np.ascontiguousarray(has_quality, dtype=np.uint8)
     q_id = np.ascontiguousarray(q_id, dtype=np.uint32)
     t_id = np.ascontiguousarray(t_id, dtype=np.uint32)
+    err = C.create_string_buffer(1024)
+    if window_length is not None:
+        t_begin = np.ascontiguousarray(t_begin, dtype=np.uint32)
+        t_end = np.ascontiguousarray(t_end, dtype=np.uint32)
+        if len(t_begin) != len(q_id) or len(t_end) != len(q_id):
+            raise ValueError("t_begin and t_end need one entry per overlap")
+        inputs = (n_targets, len(lengths), _ptr(lengths), _ptr(has_quality), len(q_id), _ptr(q_id), _ptr(t_id),
+                  _ptr(t_begin), _ptr(t_end), window_length, budget)
+        sizes = np.zeros(2, np.uint64)
+        n = lib.rp_mirror_plan_split_read_groups(*inputs, _ptr(sizes), *([None] * 7), err, len(err))
+        if n < 0:
+            raise RaconB200Error(err.value.decode(errors="replace"))
+        n_groups, n_order = int(sizes[0]), int(sizes[1])
+        out = [np.zeros(n_groups + 1, np.uint64), np.zeros(max(n_groups, 1), np.uint64),
+               np.zeros(n_groups + 1, np.uint64), np.zeros(max(n_order, 1), np.uint64),
+               np.zeros(max(n_groups, 1), np.uint32), np.zeros(max(n_groups, 1), np.uint32),
+               np.zeros(max(len(q_id), 1), np.uint64)]
+        lib.rp_mirror_plan_split_read_groups(*inputs, _ptr(sizes), *[_ptr(a) for a in out], err, len(err))
+        return (out[0], out[1][:n_groups], out[2], out[3][:n_order], out[4][:n_groups], out[5][:n_groups],
+                out[6][:len(q_id)])
     first = np.zeros(n_targets + 1, np.uint64)
     nbytes = np.zeros(max(n_targets, 1), np.uint64)
     ofirst = np.zeros(n_targets + 1, np.uint64)
     order = np.zeros(max(len(q_id), 1), np.uint64)
-    err = C.create_string_buffer(1024)
     n = lib.rp_mirror_plan_read_groups(n_targets, len(lengths), _ptr(lengths), _ptr(has_quality), len(q_id), _ptr(q_id),
                                        _ptr(t_id), budget, _ptr(first), _ptr(nbytes), _ptr(ofirst), _ptr(order), err,
                                        len(err))
@@ -796,25 +825,36 @@ def plan_read_groups(n_targets, lengths, has_quality, q_id, t_id, budget):
 
 def last_grouped_run():
     """The last polish_files run of this process (with resident_reads): rp_reads_bytes of each target group's read store,
-    and the whole-run indices of the overlaps and windows the device refused."""
+    the whole-run indices of the overlaps and windows the device refused, and per group its whole-run windows
+    [first, end) (group_windows) and the number of overlaps it sent to the aligner (group_aligned)."""
     lib = load()
     counts = np.zeros(3, np.uint64)
     lib.rp_mirror_last_grouped_run(_ptr(counts), None, None, None)
     out = [np.zeros(max(int(n), 1), np.uint64) for n in counts]
     lib.rp_mirror_last_grouped_run(_ptr(counts), *[_ptr(a) for a in out])
-    return {k: [int(v) for v in a[:int(n)]]
-            for k, a, n in zip(("group_bytes", "failed_overlaps", "failed_windows"), out, counts)}
+    run = {k: [int(v) for v in a[:int(n)]]
+           for k, a, n in zip(("group_bytes", "failed_overlaps", "failed_windows"), out, counts)}
+    n_groups = int(counts[0])
+    windows, aligned = np.zeros(max(2 * n_groups, 1), np.uint64), np.zeros(max(n_groups, 1), np.uint64)
+    lib.rp_mirror_last_grouped_run_windows(_ptr(windows), _ptr(aligned))
+    run["group_windows"] = [(int(windows[2 * g]), int(windows[2 * g + 1])) for g in range(n_groups)]
+    run["group_aligned"] = [int(v) for v in aligned[:n_groups]]
+    return run
 
 
 def polish_files(reads, overlaps, targets, out_path, fragment_correction=False, window_length=500, quality_threshold=10.0,
                  error_threshold=0.3, trim=True, match=3, mismatch=-5, gap=-4, device=0, drop_unpolished=True,
-                 mem_bytes=0, banded=False, resident_reads=True, read_store_bytes=0):
+                 mem_bytes=0, banded=False, resident_reads=True, read_store_bytes=0, split_targets=False):
     """racon's whole run through the C++ host layer: files in, polished FASTA out (alignment, breaking points and
     consensus on the device).  device: a CUDA device index or a sequence of them — device=range(device_count()) runs on
     every visible GPU; the file is byte-identical whatever the list.  With resident_reads (the default) the targets are
     polished in consecutive groups whose sequences fit a device read store of read_store_bytes per device (0 = half of
-    the smallest free device memory); the file is the same whatever the groups.  Returns (records written, overlaps the
-    device refused, windows the device refused)."""
+    the smallest free device memory); the file is the same whatever the groups.  A target whose own sequences do not fit
+    is an error, or with split_targets is polished in parts of consecutive windows that fit (plan_read_groups with the
+    window length), with the same file.  Returns (records written, overlaps the device refused, windows the device
+    refused)."""
+    if split_targets and not resident_reads:
+        raise ValueError("split_targets polishes in target groups, which need resident_reads")
     if resident_reads:
         lib = load()
         devices = _device_list(device)
@@ -824,7 +864,7 @@ def polish_files(reads, overlaps, targets, out_path, fragment_correction=False, 
             os.fsencode(reads), os.fsencode(overlaps), os.fsencode(targets), 1 if fragment_correction else 0,
             window_length, quality_threshold, error_threshold, 1 if trim else 0, match, mismatch, gap, _ptr(devices),
             len(devices), 1 if drop_unpolished else 0, mem_bytes, 1 if banded else 0, read_store_bytes,
-            os.fsencode(out_path), _ptr(result), err, len(err))
+            1 if split_targets else 0, os.fsencode(out_path), _ptr(result), err, len(err))
         if st != 0:
             raise RaconB200Error(err.value.decode(errors="replace"))
         return tuple(int(v) for v in result)

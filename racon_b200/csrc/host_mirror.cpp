@@ -393,7 +393,7 @@ const char* Polisher::reverse_quality(uint32_t id) {
     return s.quality ? r.data() : nullptr;
 }
 
-void Polisher::find_overlap_breaking_points(std::vector<Overlap>& overlaps) {
+size_t Polisher::find_overlap_breaking_points(std::vector<Overlap>& overlaps) {
     /* an overlap that came with an alignment (SAM input) keeps it, as in Overlap::find_breaking_points
      * (overlap.cpp:186-203); only the others are aligned, in batches, on the device */
     std::vector<size_t> todo;
@@ -410,9 +410,10 @@ void Polisher::find_overlap_breaking_points(std::vector<Overlap>& overlaps) {
             longest = std::max(longest, std::max(o.q_end - o.q_begin, o.t_end - o.t_begin));
         }
     }
-    if (todo.empty()) return;
+    if (todo.empty()) return 0;
     run_stage([&] { align(overlaps, todo, longest); }, [&] { release_read_stores(); });
     std::sort(failed_overlaps_.begin(), failed_overlaps_.end());   // lanes finish in any order
+    return todo.size();
 }
 
 void Polisher::align(std::vector<Overlap>& overlaps, const std::vector<size_t>& todo, uint32_t longest) {
@@ -525,45 +526,69 @@ void Polisher::build_windows(const std::vector<Overlap>& overlaps, uint64_t firs
     for (uint64_t i = 0; i < overlaps.size(); ++i) {
         const Overlap& o = overlaps[i];
         ++targets_coverages_[o.t_id];
-        const SequenceView& sequence = sequences_[o.q_id];
-        const auto& breaking_points = o.breaking_points();
-        for (uint32_t j = 0; j + 1 < breaking_points.size(); j += 2) {
-            if (breaking_points[j + 1].second - breaking_points[j].second < 0.02 * window_length_) continue;
+        add_layers(o, id_to_first_window_id[o.t_id - first_target], 0, ~0u);
+    }
+}
 
-            const char* quality = o.strand ? reverse_quality(o.q_id) : sequence.quality;
-            if (quality != nullptr) {
-                double average_quality = 0;
-                for (uint32_t k = breaking_points[j].second; k < breaking_points[j + 1].second; ++k) {
-                    average_quality += static_cast<uint32_t>(quality[k]) - 33;
-                }
-                average_quality /= breaking_points[j + 1].second - breaking_points[j].second;
-                if (average_quality < quality_threshold_) continue;
+void Polisher::build_windows(const std::vector<Overlap>& overlaps, uint64_t target, uint32_t first_window,
+                             uint32_t end_window) {
+    const uint64_t first_window_id = windows_.size();
+    const SequenceView& tgt = sequences_[target];
+    for (uint32_t k = first_window; k < end_window; ++k) {
+        const uint32_t j = k * window_length_;
+        const uint32_t length = std::min(j + window_length_, tgt.length) - j;
+        windows_.emplace_back(createWindow(target, k, window_type_, tgt.data + j, length,
+                                           tgt.quality ? tgt.quality + j : dummy_quality_.data(), length));
+        windows_.back()->set_backbone_origin(static_cast<uint32_t>(target), j);
+    }
+    targets_coverages_.resize(targets_size_);
+    for (const Overlap& o : overlaps) add_layers(o, first_window_id, first_window, end_window);
+}
+
+void Polisher::add_layers(const Overlap& o, uint64_t first_window_id, uint32_t first_window, uint32_t end_window) {
+    const SequenceView& sequence = sequences_[o.q_id];
+    const auto& breaking_points = o.breaking_points();
+    for (uint32_t j = 0; j + 1 < breaking_points.size(); j += 2) {
+        const uint32_t window = breaking_points[j].first / window_length_;
+        if (window < first_window || window >= end_window) continue;   // another part's window
+        if (breaking_points[j + 1].second - breaking_points[j].second < 0.02 * window_length_) continue;
+
+        const char* quality = o.strand ? reverse_quality(o.q_id) : sequence.quality;
+        if (quality != nullptr) {
+            double average_quality = 0;
+            for (uint32_t k = breaking_points[j].second; k < breaking_points[j + 1].second; ++k) {
+                average_quality += static_cast<uint32_t>(quality[k]) - 33;
             }
-
-            const uint64_t window_id =
-                id_to_first_window_id[o.t_id - first_target] + breaking_points[j].first / window_length_;
-            const uint32_t window_start = (breaking_points[j].first / window_length_) * window_length_;
-            const char* data = (o.strand ? reverse_complement(o.q_id) : sequence.data) + breaking_points[j].second;
-            const uint32_t data_length = breaking_points[j + 1].second - breaking_points[j].second;
-            const char* layer_quality = quality == nullptr ? nullptr : quality + breaking_points[j].second;
-            const uint32_t quality_length = quality == nullptr ? 0 : data_length;
-
-            windows_[window_id]->add_layer(data, data_length, layer_quality, quality_length,
-                                           breaking_points[j].first - window_start,
-                                           breaking_points[j + 1].first - window_start - 1,
-                                           Window::Origin{o.q_id, breaking_points[j].second, o.strand != 0});
+            average_quality /= breaking_points[j + 1].second - breaking_points[j].second;
+            if (average_quality < quality_threshold_) continue;
         }
+
+        const uint64_t window_id = first_window_id + (window - first_window);
+        const uint32_t window_start = window * window_length_;
+        const char* data = (o.strand ? reverse_complement(o.q_id) : sequence.data) + breaking_points[j].second;
+        const uint32_t data_length = breaking_points[j + 1].second - breaking_points[j].second;
+        const char* layer_quality = quality == nullptr ? nullptr : quality + breaking_points[j].second;
+        const uint32_t quality_length = quality == nullptr ? 0 : data_length;
+
+        windows_[window_id]->add_layer(data, data_length, layer_quality, quality_length,
+                                       breaking_points[j].first - window_start,
+                                       breaking_points[j + 1].first - window_start - 1,
+                                       Window::Origin{o.q_id, breaking_points[j].second, o.strand != 0});
     }
 }
 
 void Polisher::polish(std::vector<PolishedSequence>& dst, bool drop_unpolished_sequences) {
     /* the windows are kept: their consensus stays readable (Polisher::windows) */
+    stitch_data_.clear();
+    stitch_polished_ = 0;
     consensus([&](const PolishedSequence& p) { dst.push_back(p); }, drop_unpolished_sequences, 0, false,
               resident_reads_, false);
 }
 
 void Polisher::polish_streaming(const std::function<void(const PolishedSequence&)>& sink,
                                 bool drop_unpolished_sequences, size_t memory, bool banded, bool resident_reads) {
+    stitch_data_.clear();
+    stitch_polished_ = 0;
     consensus(sink, drop_unpolished_sequences, memory, banded, resident_reads || resident_reads_, true);
 }
 
@@ -591,12 +616,14 @@ void Polisher::consensus_lanes(const std::function<void(const PolishedSequence&)
         slots[i].batch->useReadStore(resident_reads ? read_store(device) : nullptr);
     }
     std::vector<uint8_t> polished(windows_.size(), 0);   // Window::generate_consensus' flag, until stitched
-    std::string polished_data;
-    uint32_t num_polished_windows = 0;
+    std::string& polished_data = stitch_data_;            // carried over when windows_ ends inside a target
+    uint32_t& num_polished_windows = stitch_polished_;
     auto stitch = [&](size_t w) {  // polisher.cpp:504-530, one window at a time, in window order
         num_polished_windows += polished[w];
         polished_data += windows_[w]->consensus();
-        if (w == windows_.size() - 1 || windows_[w + 1]->rank() == 0) {
+        const uint64_t target_length = sequences_[windows_[w]->id()].length;
+        /* the target's last window (racon: the last window of all, or one followed by a rank-0 window) */
+        if ((static_cast<uint64_t>(windows_[w]->rank()) + 1) * window_length_ >= target_length) {
             const double polished_ratio = num_polished_windows / static_cast<double>(windows_[w]->rank() + 1);
             if (!drop_unpolished_sequences || polished_ratio > 0) {
                 std::string tags = fragment_correction_ ? "r" : "";
@@ -647,6 +674,11 @@ std::string over_budget(const std::string& target_name, uint64_t bytes, uint64_t
     return "[racon_b200::Polisher] error: target " + target_name + " needs a read store of " + std::to_string(bytes) +
            " bytes, over the budget of " + std::to_string(budget) + " bytes per device!";
 }
+std::string window_over_budget(const std::string& target_name, uint32_t window, uint64_t bytes, uint64_t budget) {
+    return "[racon_b200::Polisher] error: window " + std::to_string(window) + " of target " + target_name +
+           " needs a read store of " + std::to_string(bytes) + " bytes, over the budget of " + std::to_string(budget) +
+           " bytes per device!";
+}
 }  // namespace
 
 TargetOverBudget::TargetOverBudget(uint64_t target, uint64_t bytes, uint64_t budget)
@@ -657,8 +689,16 @@ std::string TargetOverBudget::message(const std::string& target_name) const {
     return over_budget(target_name, bytes, budget);
 }
 
+WindowOverBudget::WindowOverBudget(uint64_t target, uint32_t window, uint64_t bytes, uint64_t budget)
+    : TargetOverBudget(window_over_budget("#" + std::to_string(target), window, bytes, budget), target, bytes, budget),
+      window(window) {}
+
+std::string WindowOverBudget::message(const std::string& target_name) const {
+    return window_over_budget(target_name, window, bytes, budget);
+}
+
 ReadGroups plan_read_groups(uint64_t targets_size, const std::vector<SequenceView>& sequences,
-                            const std::vector<Overlap>& overlaps, uint64_t budget) {
+                            const std::vector<Overlap>& overlaps, uint64_t budget, uint32_t window_length) {
     /* the overlaps of every target, in their original order (stable counting sort by t_id) */
     std::vector<uint64_t> by_target_first(targets_size + 1, 0), by_target(overlaps.size());
     for (const Overlap& o : overlaps) ++by_target_first[o.t_id + 1];
@@ -673,19 +713,16 @@ ReadGroups plan_read_groups(uint64_t targets_size, const std::vector<SequenceVie
     std::vector<uint64_t> member_of(sequences.size(), 0);
     uint64_t sum = 0;
     bool any_quality = false;
-    std::vector<uint32_t> fresh;   // the sequences target t adds to a group
+    std::vector<uint32_t> fresh;   // the sequences target t (or a part's next window) adds to a group
     uint64_t next_sum = 0;
     bool next_quality = false;
-    /* the store bytes of group `stamp` - 1 (of `base_sum` / `base_quality` so far) with target t in it */
-    auto with_target = [&](uint64_t t, uint64_t stamp, uint64_t base_sum, bool base_quality) {
-        fresh.clear();
-        auto add = [&](uint32_t id) {
-            if (member_of[id] == stamp) return;
-            member_of[id] = stamp;
-            fresh.push_back(id);
-        };
-        add(static_cast<uint32_t>(t));
-        for (uint64_t k = by_target_first[t]; k < by_target_first[t + 1]; ++k) add(overlaps[by_target[k]].q_id);
+    auto add = [&](uint32_t id, uint64_t stamp) {
+        if (member_of[id] == stamp) return;
+        member_of[id] = stamp;
+        fresh.push_back(id);
+    };
+    /* the store bytes of base_sum / base_quality and the fresh sequences */
+    auto with_fresh = [&](uint64_t base_sum, bool base_quality) {
         next_sum = base_sum;
         next_quality = base_quality;
         for (uint32_t id : fresh) {
@@ -694,37 +731,133 @@ ReadGroups plan_read_groups(uint64_t targets_size, const std::vector<SequenceVie
         }
         return read_store_bytes(next_sum, next_quality);
     };
+    /* the store bytes of group `stamp` - 1 (of `base_sum` / `base_quality` so far) with target t in it */
+    auto with_target = [&](uint64_t t, uint64_t stamp, uint64_t base_sum, bool base_quality) {
+        fresh.clear();
+        add(static_cast<uint32_t>(t), stamp);
+        for (uint64_t k = by_target_first[t]; k < by_target_first[t + 1]; ++k) add(overlaps[by_target[k]].q_id, stamp);
+        return with_fresh(base_sum, base_quality);
+    };
+
+    /* split targets: target t's windows cut greedily into maximal parts, each a group of its own */
+    std::vector<uint8_t> split(targets_size, 0);
+    std::vector<std::vector<uint64_t>> part_overlaps;   // per group: a part's overlaps, in file order
+    auto split_target = [&](uint64_t t, uint64_t bytes) {
+        const uint64_t n_windows = (static_cast<uint64_t>(sequences[t].length) + window_length - 1) / window_length;
+        if (n_windows == 0) throw TargetOverBudget(t, bytes, budget);
+        split[t] = 1;
+        /* the windows each overlap touches, [first_w, last_w], and the overlaps by first window (in file order) */
+        const uint64_t n = by_target_first[t + 1] - by_target_first[t];
+        std::vector<uint64_t> last_w(n), starting_first(n_windows + 1, 0), starting(n);
+        std::vector<uint64_t> first_w(n);
+        for (uint64_t i = 0; i < n; ++i) {
+            const Overlap& o = overlaps[by_target[by_target_first[t] + i]];
+            first_w[i] = std::min<uint64_t>(o.t_begin / window_length, n_windows - 1);
+            last_w[i] = o.t_end > o.t_begin ? std::min<uint64_t>((o.t_end - 1) / window_length, n_windows - 1) : 0;
+            last_w[i] = std::max(last_w[i], first_w[i]);
+            ++starting_first[first_w[i] + 1];
+        }
+        for (uint64_t w = 0; w < n_windows; ++w) starting_first[w + 1] += starting_first[w];
+        {
+            std::vector<uint64_t> at(starting_first.begin(), starting_first.end() - 1);
+            for (uint64_t i = 0; i < n; ++i) starting[at[first_w[i]]++] = i;
+        }
+        std::vector<uint64_t> carry;   // the last part's overlaps that also touch the next window
+        for (uint64_t a = 0; a < n_windows;) {
+            const uint64_t stamp = g.size() + 1;
+            /* window a alone: the target, the overlaps carried over the part boundary and those starting at a */
+            fresh.clear();
+            add(static_cast<uint32_t>(t), stamp);
+            for (uint64_t i : carry) add(overlaps[by_target[by_target_first[t] + i]].q_id, stamp);
+            for (uint64_t s = starting_first[a]; s < starting_first[a + 1]; ++s)
+                add(overlaps[by_target[by_target_first[t] + starting[s]]].q_id, stamp);
+            uint64_t part_bytes = with_fresh(0, false);
+            if (part_bytes > budget) throw WindowOverBudget(t, static_cast<uint32_t>(a), part_bytes, budget);
+            uint64_t part_sum = next_sum;
+            bool part_quality = next_quality;
+            uint64_t b = a + 1;
+            for (; b < n_windows; ++b) {   // grow while the next window's new reads fit
+                fresh.clear();
+                for (uint64_t s = starting_first[b]; s < starting_first[b + 1]; ++s)
+                    add(overlaps[by_target[by_target_first[t] + starting[s]]].q_id, stamp);
+                const uint64_t grown = with_fresh(part_sum, part_quality);
+                if (grown > budget) break;
+                part_bytes = grown;
+                part_sum = next_sum;
+                part_quality = next_quality;
+            }
+            std::vector<uint64_t> local(carry);
+            for (uint64_t s = starting_first[a]; s < starting_first[b]; ++s) local.push_back(starting[s]);
+            std::sort(local.begin(), local.end());   // file order: by_target keeps it
+            g.first_target.push_back(t);
+            g.bytes.push_back(part_bytes);
+            g.first_window.push_back(static_cast<uint32_t>(a));
+            g.end_window.push_back(static_cast<uint32_t>(b));
+            part_overlaps.resize(g.size());
+            carry.clear();
+            for (uint64_t i : local) {
+                part_overlaps.back().push_back(by_target[by_target_first[t] + i]);
+                if (last_w[i] >= b) carry.push_back(i);
+            }
+            a = b;
+        }
+    };
+
+    bool open = false;   // the last group takes further targets
     for (uint64_t t = 0; t < targets_size; ++t) {
-        const bool open = g.size() > 0;
         uint64_t bytes = open ? with_target(t, g.size(), sum, any_quality) : 0;
         if (!open || bytes > budget) {   // t starts a group of its own
             for (uint32_t id : fresh) member_of[id] = 0;
             bytes = with_target(t, g.size() + 1, 0, false);
-            if (bytes > budget) throw TargetOverBudget(t, bytes, budget);
+            if (bytes > budget) {
+                if (window_length == 0) throw TargetOverBudget(t, bytes, budget);
+                for (uint32_t id : fresh) member_of[id] = 0;   // the first part takes the stamp t tried
+                split_target(t, bytes);
+                open = false;
+                continue;
+            }
             g.first_target.push_back(t);
             g.bytes.push_back(0);
+            g.first_window.push_back(0);
+            g.end_window.push_back(0);
+            open = true;
         }
         g.bytes.back() = bytes;
         sum = next_sum;
         any_quality = next_quality;
     }
     g.first_target.push_back(targets_size);
+    part_overlaps.resize(g.size());
 
-    /* each group's overlaps in their original order (stable counting sort by group) */
+    /* each group's overlaps in their original order: a whole group's by a stable counting sort by group, a part's as
+     * planned; an overlap is aligned by its only group, or by the first part it is in */
     std::vector<uint64_t> group_of(targets_size);
     for (size_t k = 0; k < g.size(); ++k)
         std::fill(group_of.begin() + g.first_target[k], group_of.begin() + g.first_target[k + 1], k);
     g.overlap_first.assign(g.size() + 1, 0);
-    for (const Overlap& o : overlaps) ++g.overlap_first[group_of[o.t_id] + 1];
-    for (size_t k = 0; k < g.size(); ++k) g.overlap_first[k + 1] += g.overlap_first[k];
-    g.overlap_order.resize(overlaps.size());
+    for (const Overlap& o : overlaps)
+        if (!split[o.t_id]) ++g.overlap_first[group_of[o.t_id] + 1];
+    for (size_t k = 0; k < g.size(); ++k) g.overlap_first[k + 1] += g.overlap_first[k] + part_overlaps[k].size();
+    g.overlap_order.resize(g.overlap_first.back());
+    g.aligned_in.assign(overlaps.size(), ~0ull);
     std::vector<uint64_t> at(g.overlap_first.begin(), g.overlap_first.end() - 1);
-    for (uint64_t k = 0; k < overlaps.size(); ++k) g.overlap_order[at[group_of[overlaps[k].t_id]]++] = k;
+    for (uint64_t k = 0; k < overlaps.size(); ++k) {
+        if (split[overlaps[k].t_id]) continue;
+        g.aligned_in[k] = group_of[overlaps[k].t_id];
+        g.overlap_order[at[g.aligned_in[k]]++] = k;
+    }
+    for (size_t p = 0; p < g.size(); ++p) {
+        for (uint64_t k : part_overlaps[p]) {
+            if (g.aligned_in[k] == ~0ull) g.aligned_in[k] = p;
+            g.overlap_order[at[p]++] = k;
+        }
+    }
     return g;
 }
 
 void Polisher::polish_groups(std::vector<Overlap>& overlaps, const std::function<void(const PolishedSequence&)>& sink,
-                             bool drop_unpolished_sequences, size_t memory, bool banded, uint64_t read_store_bytes) {
+                             bool drop_unpolished_sequences, size_t memory, bool banded, uint64_t read_store_bytes,
+                             bool split_targets) {
     std::vector<uint32_t> distinct;
     for (uint32_t d : devices_)
         if (std::find(distinct.begin(), distinct.end(), d) == distinct.end()) distinct.push_back(d);
@@ -738,14 +871,27 @@ void Polisher::polish_groups(std::vector<Overlap>& overlaps, const std::function
         }
         read_store_bytes = smallest / 2;
     }
-    const ReadGroups groups = plan_read_groups(targets_size_, sequences_, overlaps, read_store_bytes);
+    const ReadGroups groups =
+        plan_read_groups(targets_size_, sequences_, overlaps, read_store_bytes, split_targets ? window_length_ : 0);
 
     resident_reads_ = true;
     group_store_bytes_.clear();
+    group_windows_.clear();
+    group_aligned_.clear();
+    stitch_data_.clear();
+    stitch_polished_ = 0;
+    /* RC:i: counts every overlap onto a target, whichever parts of it they touch (a whole group recounts the same) */
+    targets_coverages_.assign(targets_size_, 0);
+    for (const Overlap& o : overlaps) ++targets_coverages_[o.t_id];
+    std::vector<uint64_t> last_group(overlaps.size(), 0);   // the last group an overlap is in
+    for (size_t g = 0; g < groups.size(); ++g)
+        for (uint64_t k = groups.overlap_first[g]; k < groups.overlap_first[g + 1]; ++k)
+            last_group[groups.overlap_order[k]] = g;
     std::vector<size_t> failed_overlaps, failed_windows;   // whole-run indices
     uint64_t windows_before = 0;                           // windows of the groups before this one
     for (size_t g = 0; g < groups.size(); ++g) {
-        const uint64_t first = groups.first_target[g], end = groups.first_target[g + 1];
+        const uint64_t first = groups.first_target[g];
+        const uint64_t end = groups.is_part(g) ? first + 1 : groups.first_target[g + 1];
         /* the group's overlaps, in their original order, moved out and back */
         std::vector<Overlap> subset;
         subset.reserve(groups.overlap_first[g + 1] - groups.overlap_first[g]);
@@ -762,21 +908,42 @@ void Polisher::polish_groups(std::vector<Overlap>& overlaps, const std::function
         }, [&] { release_read_stores(); });
         group_store_bytes_.push_back(rp_reads_bytes(stores_.front().second));
 
+        /* the overlaps this group aligns: every one of a whole group, those of a part that no earlier part aligned (an
+         * overlap the device refused, or one without a match in any window, has no breaking points either) */
+        std::vector<Overlap> todo;
+        std::vector<uint64_t> todo_ids;
+        for (uint64_t k = 0; k < subset.size(); ++k) {
+            if (groups.aligned_in[global_overlap(k)] != g) continue;
+            todo.push_back(std::move(subset[k]));
+            todo_ids.push_back(global_overlap(k));
+        }
         failed_overlaps_.clear();
-        overlap_ids_ = groups.overlap_order.data() + groups.overlap_first[g];   // warnings name whole-run indices
-        find_overlap_breaking_points(subset);
+        overlap_ids_ = todo_ids.data();   // warnings name whole-run indices
+        group_aligned_.push_back(find_overlap_breaking_points(todo));
         overlap_ids_ = nullptr;
-        for (size_t k : failed_overlaps_) failed_overlaps.push_back(global_overlap(k));
+        for (size_t k : failed_overlaps_) failed_overlaps.push_back(todo_ids[k]);
+        for (uint64_t k = 0, j = 0; k < subset.size(); ++k)
+            if (groups.aligned_in[global_overlap(k)] == g) subset[k] = std::move(todo[j++]);
 
         windows_.clear();
-        build_windows(subset, first, end);
+        if (groups.is_part(g)) {
+            build_windows(subset, first, groups.first_window[g], groups.end_window[g]);
+        } else {
+            build_windows(subset, first, end);
+        }
         failed_windows_.clear();
         consensus(sink, drop_unpolished_sequences, memory, banded, true, true);
         for (size_t w : failed_windows_) failed_windows.push_back(windows_before + w);
+        group_windows_.emplace_back(windows_before, windows_before + windows_.size());
         windows_before += windows_.size();
 
         release_read_stores();
-        for (uint64_t k = 0; k < subset.size(); ++k) overlaps[global_overlap(k)] = std::move(subset[k]);
+        for (uint64_t k = 0; k < subset.size(); ++k) {
+            /* a split target's overlap is done with its breaking points after its last part */
+            if (groups.is_part(g) && last_group[global_overlap(k)] == g)
+                std::vector<std::pair<uint32_t, uint32_t>>().swap(subset[k].breaking_points_);
+            overlaps[global_overlap(k)] = std::move(subset[k]);
+        }
     }
     store_members_.clear();
     windows_.clear();
@@ -1004,17 +1171,20 @@ extern "C" void rp_mirror_polisher_close(void* hv) { delete static_cast<PolHandl
 namespace {
 /* the last rp_mirror_polish_files_grouped (rp_mirror_last_grouped_run) */
 std::vector<uint64_t> g_last_group_store_bytes, g_last_failed_overlaps, g_last_failed_windows;
+std::vector<uint64_t> g_last_group_windows, g_last_group_aligned;
 }  // namespace
 
 /* racon's whole run on files in target groups (Polisher::polish_groups): load_input, plan, polish, FASTA into `path`.
- * read_store_bytes: budget per device (0 = automatic).  result[0] = records written, [1] overlaps and [2] windows the
- * device refused.  Returns 0, or -1 with the message in err (input error, a target over the budget, unwritable path). */
+ * read_store_bytes: budget per device (0 = automatic); split_targets: polish a target over it in parts.  result[0] =
+ * records written, [1] overlaps and [2] windows the device refused.  Returns 0, or -1 with the message in err (input
+ * error, a target or window over the budget, unwritable path). */
 extern "C" int rp_mirror_polish_files_grouped(const char* reads, const char* overlaps, const char* targets,
                                               int fragment_correction, uint32_t window_length, double quality_threshold,
                                               double error_threshold, int trim, int8_t match, int8_t mismatch, int8_t gap,
                                               const uint32_t* devices, uint32_t n_devices, int drop_unpolished,
                                               uint64_t mem_bytes, int banded, uint64_t read_store_bytes,
-                                              const char* path, uint64_t* result, char* err, uint32_t err_cap) {
+                                              int split_targets, const char* path, uint64_t* result, char* err,
+                                              uint32_t err_cap) {
     using namespace racon_b200;
     auto error = [&](const std::string& what) {
         if (err && err_cap) {
@@ -1042,14 +1212,21 @@ extern "C" int rp_mirror_polish_files_grouped(const char* reads, const char* ove
                                    std::fwrite(rec.data(), 1, rec.size(), f);
                                    ++n;
                                },
-                               drop_unpolished != 0, static_cast<size_t>(mem_bytes), banded != 0, read_store_bytes);
-    } catch (const TargetOverBudget& e) {   // planned before any record: no output
+                               drop_unpolished != 0, static_cast<size_t>(mem_bytes), banded != 0, read_store_bytes,
+                               split_targets != 0);
+    } catch (const TargetOverBudget& e) {   // planned before any record: no output (WindowOverBudget too)
         std::fclose(f);
         std::remove(path);
         return error(e.message(input.sequences[e.target].name));
     }
     std::fclose(f);
     g_last_group_store_bytes = polisher.group_store_bytes();
+    g_last_group_windows.clear();
+    for (const auto& w : polisher.group_windows()) {
+        g_last_group_windows.push_back(w.first);
+        g_last_group_windows.push_back(w.second);
+    }
+    g_last_group_aligned = polisher.group_aligned();
     g_last_failed_overlaps.assign(polisher.failed_overlaps().begin(), polisher.failed_overlaps().end());
     g_last_failed_windows.assign(polisher.failed_windows().begin(), polisher.failed_windows().end());
     result[0] = n;
@@ -1068,6 +1245,13 @@ extern "C" void rp_mirror_last_grouped_run(uint64_t* counts, uint64_t* group_byt
     if (group_bytes) std::copy(g_last_group_store_bytes.begin(), g_last_group_store_bytes.end(), group_bytes);
     if (failed_overlaps) std::copy(g_last_failed_overlaps.begin(), g_last_failed_overlaps.end(), failed_overlaps);
     if (failed_windows) std::copy(g_last_failed_windows.begin(), g_last_failed_windows.end(), failed_windows);
+}
+
+/* The same run, per group (counts[0] of rp_mirror_last_grouped_run of them): its whole-run windows
+ * [group_windows[2 g], group_windows[2 g + 1]) and the number of overlaps it sent to the aligner. */
+extern "C" void rp_mirror_last_grouped_run_windows(uint64_t* group_windows, uint64_t* group_aligned) {
+    std::copy(g_last_group_windows.begin(), g_last_group_windows.end(), group_windows);
+    std::copy(g_last_group_aligned.begin(), g_last_group_aligned.end(), group_aligned);
 }
 
 /* Host-only hook of plan_read_groups: n_seq sequences (the first n_targets are the targets) of length[i], with a quality
@@ -1095,6 +1279,55 @@ extern "C" int64_t rp_mirror_plan_read_groups(uint64_t n_targets, uint32_t n_seq
         std::copy(g.bytes.begin(), g.bytes.end(), bytes);
         std::copy(g.overlap_first.begin(), g.overlap_first.end(), overlap_first);
         std::copy(g.overlap_order.begin(), g.overlap_order.end(), overlap_order);
+        return static_cast<int64_t>(g.size());
+    } catch (const std::exception& e) {
+        if (err && err_cap) {
+            std::strncpy(err, e.what(), err_cap - 1);
+            err[err_cap - 1] = '\0';
+        }
+        return -1;
+    }
+}
+
+/* Host-only hook of plan_read_groups with split targets: rp_mirror_plan_read_groups' inputs plus each overlap's target
+ * span [t_begin[k], t_end[k]) and the window length.  sizes[0] = groups, sizes[1] = entries of overlap_order (an
+ * overlap is in every part it touches); with every output NULL only sizes is written.  Outputs as
+ * rp_mirror_plan_read_groups', and per group the windows [first_window[g], end_window[g]) of a part (0, 0 for whole targets), per overlap the group that
+ * aligns it.  Returns the number of groups, or -1 with the error in err (a target with no window, or a window, over the
+ * budget). */
+extern "C" int64_t rp_mirror_plan_split_read_groups(uint64_t n_targets, uint32_t n_seq, const uint32_t* length,
+                                                    const uint8_t* has_quality, uint64_t n_overlaps,
+                                                    const uint32_t* q_id, const uint32_t* t_id,
+                                                    const uint32_t* t_begin, const uint32_t* t_end,
+                                                    uint32_t window_length, uint64_t budget, uint64_t* sizes,
+                                                    uint64_t* first_target, uint64_t* bytes, uint64_t* overlap_first,
+                                                    uint64_t* overlap_order, uint32_t* first_window,
+                                                    uint32_t* end_window, uint64_t* aligned_in, char* err,
+                                                    uint32_t err_cap) {
+    using namespace racon_b200;
+    static const char kQuality[] = "";
+    std::vector<SequenceView> seqs(n_seq);
+    for (uint32_t i = 0; i < n_seq; ++i) seqs[i] = SequenceView{nullptr, has_quality[i] ? kQuality : nullptr, length[i]};
+    std::vector<Overlap> ovl(n_overlaps);
+    for (uint64_t k = 0; k < n_overlaps; ++k) {
+        ovl[k].q_id = q_id[k];
+        ovl[k].t_id = t_id[k];
+        ovl[k].t_begin = t_begin[k];
+        ovl[k].t_end = t_end[k];
+    }
+    try {
+        const ReadGroups g = plan_read_groups(n_targets, seqs, ovl, budget, window_length);
+        sizes[0] = g.size();
+        sizes[1] = g.overlap_order.size();
+        if (first_target) {
+            std::copy(g.first_target.begin(), g.first_target.end(), first_target);
+            std::copy(g.bytes.begin(), g.bytes.end(), bytes);
+            std::copy(g.overlap_first.begin(), g.overlap_first.end(), overlap_first);
+            std::copy(g.overlap_order.begin(), g.overlap_order.end(), overlap_order);
+            std::copy(g.first_window.begin(), g.first_window.end(), first_window);
+            std::copy(g.end_window.begin(), g.end_window.end(), end_window);
+            std::copy(g.aligned_in.begin(), g.aligned_in.end(), aligned_in);
+        }
         return static_cast<int64_t>(g.size());
     } catch (const std::exception& e) {
         if (err && err_cap) {

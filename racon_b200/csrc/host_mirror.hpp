@@ -225,27 +225,50 @@ private:
 uint64_t read_store_bytes(uint64_t sum_of_lengths, bool any_quality);
 
 struct ReadGroups {
-    std::vector<uint64_t> first_target;    // group g = targets [first_target[g], first_target[g + 1])
+    /* group g = targets [first_target[g], first_target[g + 1]); a part (below) is of target first_target[g] */
+    std::vector<uint64_t> first_target;
     std::vector<uint64_t> bytes;           // predicted rp_reads_bytes of group g's store
     /* group g's overlaps, as indices into the overlaps, in their original (file) order: a window's layer order is the
      * order of its overlaps, and it decides the consensus */
     std::vector<uint64_t> overlap_first;   // group g = overlap_order[overlap_first[g] .. overlap_first[g + 1])
     std::vector<uint64_t> overlap_order;
+    /* A part (split targets only): group g is windows [first_window[g], end_window[g]) of its one target, and its
+     * overlaps are those whose target span touches one of them — an overlap across two parts is in both.  A group of
+     * whole targets has first_window[g] = end_window[g] = 0. */
+    std::vector<uint32_t> first_window, end_window;
+    /* the group that aligns overlap k: the only group it is in, or the first part it touches */
+    std::vector<uint64_t> aligned_in;
     size_t size() const { return bytes.size(); }
+    bool is_part(size_t g) const { return end_window[g] > 0; }
 };
 
-/* A single target whose own store exceeds the budget: it cannot be polished under that budget. */
+/* A single target whose own store exceeds the budget: it cannot be polished under that budget in one group. */
 struct TargetOverBudget : std::runtime_error {
     uint64_t target, bytes, budget;
     TargetOverBudget(uint64_t target, uint64_t bytes, uint64_t budget);
-    std::string message(const std::string& target_name) const;
+    TargetOverBudget(const std::string& what, uint64_t target, uint64_t bytes, uint64_t budget)
+        : std::runtime_error(what), target(target), bytes(bytes), budget(budget) {}
+    virtual ~TargetOverBudget() = default;
+    virtual std::string message(const std::string& target_name) const;
+};
+
+/* With split targets: one window of a target (the target and the reads touching that window) exceeds the budget, so no
+ * part can hold it. */
+struct WindowOverBudget : TargetOverBudget {
+    uint32_t window;
+    WindowOverBudget(uint64_t target, uint32_t window, uint64_t bytes, uint64_t budget);
+    std::string message(const std::string& target_name) const override;
 };
 
 /* Greedy over the targets in order: a group is closed when its next target would push its store over `budget` bytes.
  * Host only.  Reads sequences[i].length and whether sequences[i].quality is set, and t_id / q_id of every overlap.
- * Throws TargetOverBudget. */
+ * Throws TargetOverBudget.
+ * window_length > 0 splits targets: a target whose own store exceeds the budget closes the open group and is cut into
+ * maximal parts of consecutive windows (window_length bases each, as the polisher builds them), each a group of its
+ * own; an overlap touches windows t_begin / window_length .. (t_end - 1) / window_length.  Targets that fit get the
+ * groups they get without splitting.  Throws WindowOverBudget when one window does not fit. */
 ReadGroups plan_read_groups(uint64_t targets_size, const std::vector<SequenceView>& sequences,
-                            const std::vector<Overlap>& overlaps, uint64_t budget);
+                            const std::vector<Overlap>& overlaps, uint64_t budget, uint32_t window_length = 0);
 
 /* The polisher runs its two device stages on a list of devices: one lane per entry (the same device may appear more than
  * once: {0, 0} = two lanes on one GPU).  The aligner has one batch object per lane, the consensus two; one host thread
@@ -267,12 +290,17 @@ public:
      * their inputs instead of copying them — the aligner its two spans per overlap (rp_aln_add_overlap_ref), the consensus
      * its window pieces (rp_poa_add_window_refs).  Call before initialize(). */
     void use_resident_reads(bool on) { resident_reads_ = on; }
-    void find_overlap_breaking_points(std::vector<Overlap>& overlaps);
+    /* returns the number of overlaps sent to the device aligner */
+    size_t find_overlap_breaking_points(std::vector<Overlap>& overlaps);
     void initialize(std::vector<Overlap>& overlaps);
     /* the window-building half of initialize() alone, for overlaps whose breaking points are already known */
     void build_windows(const std::vector<Overlap>& overlaps);
     /* the same for targets [first_target, end_target) alone, whose overlaps those are */
     void build_windows(const std::vector<Overlap>& overlaps, uint64_t first_target, uint64_t end_target);
+    /* the same for windows [first_window, end_window) of one target alone, from the overlaps that touch them: layers
+     * that fall in the target's other windows are left out, and the target's RC:i: count is not touched */
+    void build_windows(const std::vector<Overlap>& overlaps, uint64_t target, uint32_t first_window,
+                       uint32_t end_window);
     void polish(std::vector<PolishedSequence>& dst, bool drop_unpolished_sequences);
     /* Streaming form (polisher.cpp:504-537 + main.cpp:159-161 as a consumer overlapped with the compute): two batch
      * objects per lane stay in flight; while they run on the GPUs the finished windows are stitched in window order, and
@@ -287,11 +315,20 @@ public:
      * streamed to `sink`, and its store released.  `read_store_bytes` = budget per device (0 = half of the smallest free
      * memory of the devices, read before anything is allocated).  The overlaps come from load_input (filter and window
      * type over the whole input); failed_overlaps / failed_windows keep their whole-run indices.  With one group the
-     * output is that of initialize + polish_streaming.  Throws TargetOverBudget before any device work. */
+     * output is that of initialize + polish_streaming.  Throws TargetOverBudget before any device work.
+     * split_targets: a target whose own store exceeds the budget is polished in parts (plan_read_groups with the window
+     * length): each overlap is aligned once, in the first part it touches, and keeps its breaking points until its last
+     * part has built its windows; a part builds only its windows, and the target's record is stitched across its parts
+     * and goes to `sink` after its last window, with RC:i: counting every overlap onto the target.  The output is still
+     * that of one pass.  Throws WindowOverBudget (before any device work) when one window does not fit. */
     void polish_groups(std::vector<Overlap>& overlaps, const std::function<void(const PolishedSequence&)>& sink,
-                       bool drop_unpolished_sequences, size_t memory, bool banded, uint64_t read_store_bytes);
+                       bool drop_unpolished_sequences, size_t memory, bool banded, uint64_t read_store_bytes,
+                       bool split_targets = false);
     /* rp_reads_bytes of each group's store in the last polish_groups (of the first device's copy) */
     const std::vector<uint64_t>& group_store_bytes() const { return group_store_bytes_; }
+    /* per group of the last polish_groups: its whole-run windows [first, end), and how many overlaps it aligned */
+    const std::vector<std::pair<uint64_t, uint64_t>>& group_windows() const { return group_windows_; }
+    const std::vector<uint64_t>& group_aligned() const { return group_aligned_; }
     const std::vector<std::shared_ptr<Window>>& windows() const { return windows_; }
     /* Items the device could not finish (soft RP_ALN_* / RP_WIN_* status).  The reference hands such items to its CPU
      * code (cudapolisher.cpp:213 edlib, :354-370 spoa); this library has no CPU path, so a failed overlap contributes
@@ -315,6 +352,9 @@ private:
     void consensus_lanes(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
                          size_t memory, bool banded, bool resident_reads, bool release);
     void release_read_stores();
+    /* the layers of overlap o in windows [first_window, end_window) of its target, whose window first_window is
+     * windows_[first_window_id] (polisher.cpp:405-458) */
+    void add_layers(const Overlap& o, uint64_t first_window_id, uint32_t first_window, uint32_t end_window);
 
     std::vector<SequenceView> sequences_;
     uint64_t targets_size_;
@@ -333,7 +373,11 @@ private:
     bool resident_reads_ = false;
     std::vector<std::pair<uint32_t, rp_reads*>> stores_;   // (device, store): one per distinct device, made at first use
     std::vector<uint8_t> store_members_;   // empty: stores hold every sequence; else those i with store_members_[i]
-    std::vector<uint64_t> group_store_bytes_;
+    std::vector<uint64_t> group_store_bytes_, group_aligned_;
+    std::vector<std::pair<uint64_t, uint64_t>> group_windows_;
+    /* the stitch of the target whose windows are being emitted: it carries from one part of a split target to the next */
+    std::string stitch_data_;
+    uint32_t stitch_polished_ = 0;
     const uint64_t* overlap_ids_ = nullptr;   // while a group is aligned: whole-run index of each overlap of the group
     const rp_reads* read_store(uint32_t device);
 };

@@ -7,10 +7,11 @@
  * atof conversions, int8_t scores, `-c` taking its count from the next word when that word is not an option).  The run is
  * the host layer's: load_input (parsing + racon's overlap filter), then Polisher on every visible GPU (alignment,
  * breaking points and consensus on the device) in target groups whose sequences fit the device read store budget
- * (polish_groups, RP_READ_STORE_BYTES), whose sink writes each record to stdout the moment it is stitched.
+ * (polish_groups, RP_READ_STORE_BYTES; with --split-targets a target that does not fit on its own is polished in window
+ * ranges that do), whose sink writes each record to stdout the moment it is stitched.
  *
- * Exit status: 0 = racon's bytes; 1 = an error (bad argument, bad input, no device, a target over the read store budget, a device error,
- * a failed write);
+ * Exit status: 0 = racon's bytes; 1 = an error (bad argument, bad input, no device, a target over the read store budget
+ * (with --split-targets: a window over it), a device error, a failed write);
  * 2 = the output was written, but the device refused some overlaps or windows (a soft RP_ALN_* / RP_WIN_* status).  racon
  * redoes such items on its CPU; this program has no CPU path, so its output then differs from racon's.
  */
@@ -35,6 +36,7 @@ namespace {
 
 constexpr int kCudaAlignerBatches = 10000;     // long options without a short form
 constexpr int kCudaAlignerBandWidth = 10001;
+constexpr int kSplitTargets = 10002;
 
 const struct option kOptions[] = {
     {"include-unpolished", no_argument, nullptr, 'u'},
@@ -53,6 +55,7 @@ const struct option kOptions[] = {
     {"cuda-banded-alignment", no_argument, nullptr, 'b'},
     {"cudaaligner-batches", required_argument, nullptr, kCudaAlignerBatches},
     {"cudaaligner-band-width", required_argument, nullptr, kCudaAlignerBandWidth},
+    {"split-targets", no_argument, nullptr, kSplitTargets},
     {nullptr, 0, nullptr, 0}};
 
 void usage(FILE* out) {
@@ -80,6 +83,9 @@ void usage(FILE* out) {
         "    -b, --cuda-banded-alignment    banded consensus alignment (same output wherever the band holds the optimum)\n"
         "    -c, --cudapoa-batches [<int>]  default 1: lanes per GPU; a lane is one aligner and two consensus batches\n"
         "                                   (a count below 1 is taken as 1)\n"
+        "    --split-targets                polish a target whose sequences do not fit the read store budget in\n"
+        "                                   consecutive window ranges that do, with the output of one pass; a single\n"
+        "                                   window that does not fit is an error (status 1)\n"
         "    --version                      print the library version\n"
         "    -h, --help                     print this text\n"
         "\n"
@@ -92,7 +98,8 @@ void usage(FILE* out) {
         "    RP_READ_STORE_BYTES=<bytes>    device memory per GPU for the sequences of one group of targets: the targets\n"
         "                                   are polished in consecutive groups whose sequences fit it, with the output of\n"
         "                                   one pass.  Unset or 0: half of the smallest free GPU memory.  A target whose\n"
-        "                                   own sequences do not fit is an error (status 1)\n"
+        "                                   own sequences do not fit is an error (status 1),\n"
+        "                                   unless --split-targets is given\n"
         "\n"
         "exit status: 0 = output written; 1 = error; 2 = output written, but the device refused some overlaps or\n"
         "windows, which racon would have redone on its CPU: the output then differs from racon's.\n",
@@ -133,6 +140,7 @@ int main(int argc, char** argv) {
     bool drop_unpolished_sequences = true;
     int lanes_per_device = 1;
     bool banded = false;
+    bool split_targets = false;
 
     int argument;
     while ((argument = getopt_long(argc, argv, "ufw:q:e:m:x:g:t:hbc::", kOptions, nullptr)) != -1) {
@@ -158,6 +166,7 @@ int main(int argc, char** argv) {
             case 'b': banded = true; break;
             case kCudaAlignerBatches: break;
             case kCudaAlignerBandWidth: break;
+            case kSplitTargets: split_targets = true; break;
             default: return 1;   // getopt_long has named the option on stderr
         }
     }
@@ -214,14 +223,17 @@ int main(int argc, char** argv) {
                 const std::string record = racon_b200::format_fasta(input.sequences[s.id].name, s);
                 if (fwrite(record.data(), 1, record.size(), stdout) != record.size()) throw WriteError(errno);
             },
-            drop_unpolished_sequences, 0, banded, read_store_bytes);
+            drop_unpolished_sequences, 0, banded, read_store_bytes, split_targets);
         failed_overlaps = polisher.failed_overlaps().size();
         failed_windows = polisher.failed_windows().size();
     } catch (const WriteError& e) {
         fprintf(stderr, "[racon_b200::main] error: writing the output failed: %s\n", strerror(e.error));
         return 1;
-    } catch (const racon_b200::TargetOverBudget& e) {
+    } catch (const racon_b200::TargetOverBudget& e) {   // a target, or with --split-targets a window, over the budget
         fprintf(stderr, "%s\n", e.message(input.sequences[e.target].name).c_str());
+        if (!split_targets) {
+            fprintf(stderr, "[racon_b200::main] note: --split-targets polishes such a target in window ranges that fit\n");
+        }
         return 1;
     }
     if (fflush(stdout) != 0 || ferror(stdout)) {
