@@ -98,10 +98,8 @@ HOST_SIGNATURES = {
                                               _vp, _u32, _int, _u64, _int, _u64, _int, _str, _vp, _vp, _u32]),
     "rp_mirror_last_grouped_run": (None, [_vp, _vp, _vp, _vp]),
     "rp_mirror_last_grouped_run_windows": (None, [_vp, _vp]),
-    "rp_mirror_plan_read_groups": (C.c_int64, [_u64, _u32, _vp, _vp, _u64, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp,
-                                               _u32]),
-    "rp_mirror_plan_split_read_groups": (C.c_int64, [_u64, _u32, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _u32, _u64, _vp,
-                                                     _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32]),
+    "rp_mirror_plan_read_groups": (C.c_int64, [_u64, _u32, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _u32, _u64, _vp, _vp,
+                                               _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u32]),
     "rp_mirror_format_fasta": (_u64, [_str, _str, _str, _u64, _str, _u64]),
     "rp_mirror_stitch_order": (_u64, [_u32, _vp, _vp, _vp, _vp]),
     "rp_mirror_input_open": (_vp, [_str, _str, _str, _int, C.c_double, _vp, _u32]),
@@ -792,35 +790,27 @@ def plan_read_groups(n_targets, lengths, has_quality, q_id, t_id, budget, *, t_b
     q_id = np.ascontiguousarray(q_id, dtype=np.uint32)
     t_id = np.ascontiguousarray(t_id, dtype=np.uint32)
     err = C.create_string_buffer(1024)
-    if window_length is not None:
+    split = window_length is not None
+    if split:
         t_begin = np.ascontiguousarray(t_begin, dtype=np.uint32)
         t_end = np.ascontiguousarray(t_end, dtype=np.uint32)
         if len(t_begin) != len(q_id) or len(t_end) != len(q_id):
             raise ValueError("t_begin and t_end need one entry per overlap")
-        inputs = (n_targets, len(lengths), _ptr(lengths), _ptr(has_quality), len(q_id), _ptr(q_id), _ptr(t_id),
-                  _ptr(t_begin), _ptr(t_end), window_length, budget)
-        sizes = np.zeros(2, np.uint64)
-        n = lib.rp_mirror_plan_split_read_groups(*inputs, _ptr(sizes), *([None] * 7), err, len(err))
-        if n < 0:
-            raise RaconB200Error(err.value.decode(errors="replace"))
-        n_groups, n_order = int(sizes[0]), int(sizes[1])
-        out = [np.zeros(n_groups + 1, np.uint64), np.zeros(max(n_groups, 1), np.uint64),
-               np.zeros(n_groups + 1, np.uint64), np.zeros(max(n_order, 1), np.uint64),
-               np.zeros(max(n_groups, 1), np.uint32), np.zeros(max(n_groups, 1), np.uint32),
-               np.zeros(max(len(q_id), 1), np.uint64)]
-        lib.rp_mirror_plan_split_read_groups(*inputs, _ptr(sizes), *[_ptr(a) for a in out], err, len(err))
-        return (out[0], out[1][:n_groups], out[2], out[3][:n_order], out[4][:n_groups], out[5][:n_groups],
-                out[6][:len(q_id)])
-    first = np.zeros(n_targets + 1, np.uint64)
-    nbytes = np.zeros(max(n_targets, 1), np.uint64)
-    ofirst = np.zeros(n_targets + 1, np.uint64)
-    order = np.zeros(max(len(q_id), 1), np.uint64)
-    n = lib.rp_mirror_plan_read_groups(n_targets, len(lengths), _ptr(lengths), _ptr(has_quality), len(q_id), _ptr(q_id),
-                                       _ptr(t_id), budget, _ptr(first), _ptr(nbytes), _ptr(ofirst), _ptr(order), err,
-                                       len(err))
+    inputs = (n_targets, len(lengths), _ptr(lengths), _ptr(has_quality), len(q_id), _ptr(q_id), _ptr(t_id),
+              _ptr(t_begin) if split else None, _ptr(t_end) if split else None, window_length or 0, budget)
+    sizes = np.zeros(2, np.uint64)
+    n = lib.rp_mirror_plan_read_groups(*inputs, _ptr(sizes), *([None] * 7), err, len(err))
     if n < 0:
         raise RaconB200Error(err.value.decode(errors="replace"))
-    return first[:n + 1], nbytes[:n], ofirst[:n + 1], order[:len(q_id)]
+    n_groups, n_order = int(sizes[0]), int(sizes[1])
+    out = [np.zeros(n_groups + 1, np.uint64), np.zeros(max(n_groups, 1), np.uint64),
+           np.zeros(n_groups + 1, np.uint64), np.zeros(max(n_order, 1), np.uint64),
+           np.zeros(max(n_groups, 1), np.uint32), np.zeros(max(n_groups, 1), np.uint32),
+           np.zeros(max(len(q_id), 1), np.uint64)]
+    lib.rp_mirror_plan_read_groups(*inputs, _ptr(sizes), *[_ptr(a) for a in out], err, len(err))
+    plan = (out[0], out[1][:n_groups], out[2], out[3][:n_order], out[4][:n_groups], out[5][:n_groups],
+            out[6][:len(q_id)])
+    return plan if split else plan[:4]
 
 
 def last_grouped_run():

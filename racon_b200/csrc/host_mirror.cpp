@@ -4,11 +4,13 @@
 #include "host_mirror.hpp"
 
 #include <algorithm>
+#include <array>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <deque>
 #include <iterator>
+#include <numeric>
 #include <stdexcept>
 
 #include "racon_b200.h"
@@ -293,6 +295,12 @@ void run_lanes(size_t n_lanes, Fill&& fill, Ready&& ready, Drain&& drain) {
     }
 }
 
+std::vector<uint64_t> every_index(size_t n) {
+    std::vector<uint64_t> ids(n);
+    std::iota(ids.begin(), ids.end(), 0);
+    return ids;
+}
+
 /* Runs one device stage of the polisher: on a hard error anywhere inside, the stage's batch objects (its locals) are
  * destroyed while the error leaves it, then release() frees the read stores, then the process ends with the message. */
 template <typename Stage, typename Release>
@@ -318,7 +326,7 @@ Polisher::Polisher(std::vector<SequenceView> sequences, uint64_t targets_size, W
       fragment_correction_(fragment_correction), window_length_(window_length), quality_threshold_(quality_threshold),
       trim_(trim), match_(match), mismatch_(mismatch), gap_(gap), devices_(std::move(devices)),
       dummy_quality_(window_length, '!'),  // polisher.cpp:174
-      reverse_complement_(sequences_.size()), reverse_quality_(sequences_.size()) {
+      reverse_complement_(sequences_.size()), reverse_quality_(sequences_.size()), targets_coverages_(targets_size, 0) {
     if (window_length == 0) {  // polisher.cpp:71-75
         fprintf(stderr, "[racon_b200::Polisher] error: invalid window length!\n");
         exit(1);
@@ -346,13 +354,13 @@ void Polisher::release_read_stores() {
 }
 
 /* rp_reads is read-only once rp_reads_create has returned, so every batch object on `device` shares its one store */
-const rp_reads* Polisher::read_store(uint32_t device) {
+const rp_reads* Polisher::read_store(uint32_t device, const std::vector<uint8_t>& members) {
     for (const auto& s : stores_)
         if (s.first == device) return s.second;
     std::vector<const char*> data(sequences_.size()), quality(sequences_.size());
     std::vector<uint32_t> length(sequences_.size());
     for (size_t i = 0; i < sequences_.size(); ++i) {
-        if (!store_members_.empty() && !store_members_[i]) continue;   // absent: length 0, no bytes on the device
+        if (!members.empty() && !members[i]) continue;   // absent: length 0, no bytes on the device
         data[i] = sequences_[i].data;
         quality[i] = sequences_[i].quality;
         length[i] = sequences_[i].length;
@@ -394,12 +402,16 @@ const char* Polisher::reverse_quality(uint32_t id) {
 }
 
 size_t Polisher::find_overlap_breaking_points(std::vector<Overlap>& overlaps) {
+    return find_overlap_breaking_points(overlaps, every_index(overlaps.size()));
+}
+
+size_t Polisher::find_overlap_breaking_points(std::vector<Overlap>& overlaps, const std::vector<uint64_t>& ids) {
     /* an overlap that came with an alignment (SAM input) keeps it, as in Overlap::find_breaking_points
      * (overlap.cpp:186-203); only the others are aligned, in batches, on the device */
-    std::vector<size_t> todo;
-    todo.reserve(overlaps.size());
+    std::vector<uint64_t> todo;
+    todo.reserve(ids.size());
     uint32_t longest = 1;
-    for (size_t k = 0; k < overlaps.size(); ++k) {
+    for (uint64_t k : ids) {
         Overlap& o = overlaps[k];
         if (!o.breaking_points_.empty()) continue;
         if (!o.cigar.empty()) {
@@ -416,7 +428,7 @@ size_t Polisher::find_overlap_breaking_points(std::vector<Overlap>& overlaps) {
     return todo.size();
 }
 
-void Polisher::align(std::vector<Overlap>& overlaps, const std::vector<size_t>& todo, uint32_t longest) {
+void Polisher::align(std::vector<Overlap>& overlaps, const std::vector<uint64_t>& todo, uint32_t longest) {
     struct Lane {
         std::unique_ptr<rp_aln, void (*)(rp_aln*)> aln{nullptr, rp_aln_destroy};
         uint32_t device = 0;
@@ -481,8 +493,7 @@ void Polisher::align(std::vector<Overlap>& overlaps, const std::vector<size_t>& 
             if (st != RP_ALN_OK) {
                 /* the reference re-aligns such overlaps with its CPU edlib (cudapolisher.cpp:213); this path has no CPU
                  * aligner, so the overlap contributes no layers and the caller is told */
-                fprintf(stderr, "[racon_b200::Polisher] warning: overlap %zu exceeded device limit %u\n",
-                        static_cast<size_t>(overlap_ids_ ? overlap_ids_[k] : k), st);
+                fprintf(stderr, "[racon_b200::Polisher] warning: overlap %zu exceeded device limit %u\n", k, st);
                 failed_overlaps_.push_back(k);
                 continue;
             }
@@ -498,51 +509,37 @@ void Polisher::align(std::vector<Overlap>& overlaps, const std::vector<size_t>& 
 
 void Polisher::initialize(std::vector<Overlap>& overlaps) {
     find_overlap_breaking_points(overlaps);
+    count_coverages(overlaps);
     build_windows(overlaps);
 }
 
-void Polisher::build_windows(const std::vector<Overlap>& overlaps) { build_windows(overlaps, 0, targets_size_); }
+void Polisher::count_coverages(const std::vector<Overlap>& overlaps) {
+    targets_coverages_.assign(targets_size_, 0);
+    for (const Overlap& o : overlaps) ++targets_coverages_[o.t_id];
+}
 
-void Polisher::build_windows(const std::vector<Overlap>& overlaps, uint64_t first_target, uint64_t end_target) {
+void Polisher::build_windows(const std::vector<Overlap>& overlaps) {
+    build_windows(overlaps, every_index(overlaps.size()), 0, targets_size_, 0, ReadGroups::kAllWindows);
+}
 
-    /* one window per window_length_ bases of every target (polisher.cpp:383-401), appended to windows_ */
-    std::vector<uint64_t> id_to_first_window_id(end_target - first_target + 1, windows_.size());
+void Polisher::build_windows(const std::vector<Overlap>& overlaps, const std::vector<uint64_t>& ids,
+                             uint64_t first_target, uint64_t end_target, uint32_t first_window, uint32_t end_window) {
+    /* one window per window_length_ bases of every target (polisher.cpp:383-401) */
+    std::vector<uint64_t> first_window_id(end_target - first_target);
     for (uint64_t i = first_target; i < end_target; ++i) {
-        uint32_t k = 0;
         const SequenceView& tgt = sequences_[i];
-        for (uint32_t j = 0; j < tgt.length; j += window_length_, ++k) {
+        first_window_id[i - first_target] = windows_.size();
+        for (uint64_t k = first_window; k < end_window && k * window_length_ < tgt.length; ++k) {
+            const uint32_t j = static_cast<uint32_t>(k * window_length_);
             const uint32_t length = std::min(j + window_length_, tgt.length) - j;
-            windows_.emplace_back(createWindow(i, k, window_type_, tgt.data + j, length,
+            windows_.emplace_back(createWindow(i, static_cast<uint32_t>(k), window_type_, tgt.data + j, length,
                                                tgt.quality ? tgt.quality + j : dummy_quality_.data(), length));
             windows_.back()->set_backbone_origin(static_cast<uint32_t>(i), j);
         }
-        id_to_first_window_id[i - first_target + 1] = id_to_first_window_id[i - first_target] + k;
     }
-
-    targets_coverages_.resize(targets_size_);
-    std::fill(targets_coverages_.begin() + first_target, targets_coverages_.begin() + end_target, 0);
-
     /* one layer per pair of breaking points (polisher.cpp:405-458) */
-    for (uint64_t i = 0; i < overlaps.size(); ++i) {
-        const Overlap& o = overlaps[i];
-        ++targets_coverages_[o.t_id];
-        add_layers(o, id_to_first_window_id[o.t_id - first_target], 0, ~0u);
-    }
-}
-
-void Polisher::build_windows(const std::vector<Overlap>& overlaps, uint64_t target, uint32_t first_window,
-                             uint32_t end_window) {
-    const uint64_t first_window_id = windows_.size();
-    const SequenceView& tgt = sequences_[target];
-    for (uint32_t k = first_window; k < end_window; ++k) {
-        const uint32_t j = k * window_length_;
-        const uint32_t length = std::min(j + window_length_, tgt.length) - j;
-        windows_.emplace_back(createWindow(target, k, window_type_, tgt.data + j, length,
-                                           tgt.quality ? tgt.quality + j : dummy_quality_.data(), length));
-        windows_.back()->set_backbone_origin(static_cast<uint32_t>(target), j);
-    }
-    targets_coverages_.resize(targets_size_);
-    for (const Overlap& o : overlaps) add_layers(o, first_window_id, first_window, end_window);
+    for (uint64_t k : ids)
+        add_layers(overlaps[k], first_window_id[overlaps[k].t_id - first_target], first_window, end_window);
 }
 
 void Polisher::add_layers(const Overlap& o, uint64_t first_window_id, uint32_t first_window, uint32_t end_window) {
@@ -579,28 +576,27 @@ void Polisher::add_layers(const Overlap& o, uint64_t first_window_id, uint32_t f
 
 void Polisher::polish(std::vector<PolishedSequence>& dst, bool drop_unpolished_sequences) {
     /* the windows are kept: their consensus stays readable (Polisher::windows) */
-    stitch_data_.clear();
-    stitch_polished_ = 0;
-    consensus([&](const PolishedSequence& p) { dst.push_back(p); }, drop_unpolished_sequences, 0, false,
+    Stitch stitch;
+    consensus([&](const PolishedSequence& p) { dst.push_back(p); }, stitch, drop_unpolished_sequences, 0, false,
               resident_reads_, false);
 }
 
 void Polisher::polish_streaming(const std::function<void(const PolishedSequence&)>& sink,
                                 bool drop_unpolished_sequences, size_t memory, bool banded, bool resident_reads) {
-    stitch_data_.clear();
-    stitch_polished_ = 0;
-    consensus(sink, drop_unpolished_sequences, memory, banded, resident_reads || resident_reads_, true);
+    Stitch stitch;
+    consensus(sink, stitch, drop_unpolished_sequences, memory, banded, resident_reads || resident_reads_, true);
 }
 
-void Polisher::consensus(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
-                         size_t memory, bool banded, bool resident_reads, bool release) {
-    run_stage([&] { consensus_lanes(sink, drop_unpolished_sequences, memory, banded, resident_reads, release); },
+void Polisher::consensus(const std::function<void(const PolishedSequence&)>& sink, Stitch& stitch,
+                         bool drop_unpolished_sequences, size_t memory, bool banded, bool resident_reads, bool release) {
+    run_stage([&] { consensus_lanes(sink, stitch, drop_unpolished_sequences, memory, banded, resident_reads, release); },
               [&] { release_read_stores(); });
     std::sort(failed_windows_.begin(), failed_windows_.end());   // batches finish in any order
 }
 
-void Polisher::consensus_lanes(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
-                               size_t memory, bool banded, bool resident_reads, bool release) {
+void Polisher::consensus_lanes(const std::function<void(const PolishedSequence&)>& sink, Stitch& stitch,
+                               bool drop_unpolished_sequences, size_t memory, bool banded, bool resident_reads,
+                               bool release) {
     constexpr size_t kObjectsPerLane = 2;   // one runs on the device while the host fills / collects the other
     struct Slot {
         std::unique_ptr<BatchProcessor> batch;
@@ -616,9 +612,9 @@ void Polisher::consensus_lanes(const std::function<void(const PolishedSequence&)
         slots[i].batch->useReadStore(resident_reads ? read_store(device) : nullptr);
     }
     std::vector<uint8_t> polished(windows_.size(), 0);   // Window::generate_consensus' flag, until stitched
-    std::string& polished_data = stitch_data_;            // carried over when windows_ ends inside a target
-    uint32_t& num_polished_windows = stitch_polished_;
-    auto stitch = [&](size_t w) {  // polisher.cpp:504-530, one window at a time, in window order
+    std::string& polished_data = stitch.data;             // carried over when windows_ ends inside a target
+    uint32_t& num_polished_windows = stitch.polished_windows;
+    auto emit = [&](size_t w) {  // polisher.cpp:504-530, one window at a time, in window order
         num_polished_windows += polished[w];
         polished_data += windows_[w]->consensus();
         const uint64_t target_length = sequences_[windows_[w]->id()].length;
@@ -659,7 +655,7 @@ void Polisher::consensus_lanes(const std::function<void(const PolishedSequence&)
         for (uint32_t k : slot.batch->failedWindows()) failed_windows_.push_back(slot.first + k);
         for (size_t k = 0; k < slot.count; ++k) polished[slot.first + k] = flags[k] ? 1 : 0;
         slot.batch->reset();   // drops the batch's references to its windows
-        stitcher.finish(slot.first, slot.count, stitch);
+        stitcher.finish(slot.first, slot.count, emit);
     };
     run_lanes(slots.size(), fill, ready, drain);
 }
@@ -697,6 +693,49 @@ std::string WindowOverBudget::message(const std::string& target_name) const {
     return window_over_budget(target_name, window, bytes, budget);
 }
 
+namespace {
+/* The store of the group being planned: the sequences in it (stamp_of_[i] == stamp_), their summed length and whether
+ * any has a quality string. */
+class OpenStore {
+public:
+    explicit OpenStore(const std::vector<SequenceView>& sequences)
+        : sequences_(sequences), stamp_of_(sequences.size(), 0) {}
+    void open() {   // a new, empty store
+        ++stamp_;
+        joining_.clear();
+        sum_ = 0;
+        quality_ = false;
+    }
+    /* the store's bytes if sequences `ids` joined it (a sequence in it already, or named twice, counts once) */
+    uint64_t bytes_with(const std::vector<uint32_t>& ids) {
+        for (uint32_t id : joining_) stamp_of_[id] = 0;   // offered last time and not committed
+        joining_.clear();
+        joined_sum_ = sum_;
+        joined_quality_ = quality_;
+        for (uint32_t id : ids) {
+            if (stamp_of_[id] == stamp_) continue;
+            stamp_of_[id] = stamp_;
+            joining_.push_back(id);
+            joined_sum_ += sequences_[id].length;
+            joined_quality_ = joined_quality_ || (sequences_[id].quality != nullptr && sequences_[id].length > 0);
+        }
+        return read_store_bytes(joined_sum_, joined_quality_);
+    }
+    void commit() {   // the sequences of the last bytes_with join the store
+        joining_.clear();
+        sum_ = joined_sum_;
+        quality_ = joined_quality_;
+    }
+
+private:
+    const std::vector<SequenceView>& sequences_;
+    std::vector<uint64_t> stamp_of_;
+    std::vector<uint32_t> joining_;
+    uint64_t stamp_ = 0, sum_ = 0, joined_sum_ = 0;
+    bool quality_ = false, joined_quality_ = false;
+};
+}  // namespace
+
 ReadGroups plan_read_groups(uint64_t targets_size, const std::vector<SequenceView>& sequences,
                             const std::vector<Overlap>& overlaps, uint64_t budget, uint32_t window_length) {
     /* the overlaps of every target, in their original order (stable counting sort by t_id) */
@@ -707,152 +746,110 @@ ReadGroups plan_read_groups(uint64_t targets_size, const std::vector<SequenceVie
         std::vector<uint64_t> at(by_target_first.begin(), by_target_first.end() - 1);
         for (uint64_t k = 0; k < overlaps.size(); ++k) by_target[at[overlaps[k].t_id]++] = k;
     }
-
-    ReadGroups g;
-    /* the open group's store: its sequences (member_of[i] == group index + 1), their summed length, any quality */
-    std::vector<uint64_t> member_of(sequences.size(), 0);
-    uint64_t sum = 0;
-    bool any_quality = false;
-    std::vector<uint32_t> fresh;   // the sequences target t (or a part's next window) adds to a group
-    uint64_t next_sum = 0;
-    bool next_quality = false;
-    auto add = [&](uint32_t id, uint64_t stamp) {
-        if (member_of[id] == stamp) return;
-        member_of[id] = stamp;
-        fresh.push_back(id);
+    auto n_windows = [&](uint64_t t) {
+        return (static_cast<uint64_t>(sequences[t].length) + window_length - 1) / window_length;
     };
-    /* the store bytes of base_sum / base_quality and the fresh sequences */
-    auto with_fresh = [&](uint64_t base_sum, bool base_quality) {
-        next_sum = base_sum;
-        next_quality = base_quality;
-        for (uint32_t id : fresh) {
-            next_sum += sequences[id].length;
-            next_quality = next_quality || (sequences[id].quality != nullptr && sequences[id].length > 0);
-        }
-        return read_store_bytes(next_sum, next_quality);
-    };
-    /* the store bytes of group `stamp` - 1 (of `base_sum` / `base_quality` so far) with target t in it */
-    auto with_target = [&](uint64_t t, uint64_t stamp, uint64_t base_sum, bool base_quality) {
-        fresh.clear();
-        add(static_cast<uint32_t>(t), stamp);
-        for (uint64_t k = by_target_first[t]; k < by_target_first[t + 1]; ++k) add(overlaps[by_target[k]].q_id, stamp);
-        return with_fresh(base_sum, base_quality);
+    /* the windows [first, last] of its target that overlap o touches (all at 0 without a window length) */
+    auto touched = [&](const Overlap& o) -> std::pair<uint64_t, uint64_t> {
+        if (window_length == 0) return {0, 0};
+        const uint64_t last_window = std::max<uint64_t>(n_windows(o.t_id), 1) - 1;
+        const uint64_t first = std::min<uint64_t>(o.t_begin / window_length, last_window);
+        const uint64_t last = o.t_end > o.t_begin ? std::min<uint64_t>((o.t_end - 1) / window_length, last_window) : 0;
+        return {first, std::max(first, last)};
     };
 
-    /* split targets: target t's windows cut greedily into maximal parts, each a group of its own */
-    std::vector<uint8_t> split(targets_size, 0);
-    std::vector<std::vector<uint64_t>> part_overlaps;   // per group: a part's overlaps, in file order
-    auto split_target = [&](uint64_t t, uint64_t bytes) {
-        const uint64_t n_windows = (static_cast<uint64_t>(sequences[t].length) + window_length - 1) / window_length;
-        if (n_windows == 0) throw TargetOverBudget(t, bytes, budget);
-        split[t] = 1;
-        /* the windows each overlap touches, [first_w, last_w], and the overlaps by first window (in file order) */
-        const uint64_t n = by_target_first[t + 1] - by_target_first[t];
-        std::vector<uint64_t> last_w(n), starting_first(n_windows + 1, 0), starting(n);
-        std::vector<uint64_t> first_w(n);
-        for (uint64_t i = 0; i < n; ++i) {
-            const Overlap& o = overlaps[by_target[by_target_first[t] + i]];
-            first_w[i] = std::min<uint64_t>(o.t_begin / window_length, n_windows - 1);
-            last_w[i] = o.t_end > o.t_begin ? std::min<uint64_t>((o.t_end - 1) / window_length, n_windows - 1) : 0;
-            last_w[i] = std::max(last_w[i], first_w[i]);
-            ++starting_first[first_w[i] + 1];
-        }
-        for (uint64_t w = 0; w < n_windows; ++w) starting_first[w + 1] += starting_first[w];
-        {
-            std::vector<uint64_t> at(starting_first.begin(), starting_first.end() - 1);
-            for (uint64_t i = 0; i < n; ++i) starting[at[first_w[i]]++] = i;
-        }
-        std::vector<uint64_t> carry;   // the last part's overlaps that also touch the next window
-        for (uint64_t a = 0; a < n_windows;) {
-            const uint64_t stamp = g.size() + 1;
-            /* window a alone: the target, the overlaps carried over the part boundary and those starting at a */
-            fresh.clear();
-            add(static_cast<uint32_t>(t), stamp);
-            for (uint64_t i : carry) add(overlaps[by_target[by_target_first[t] + i]].q_id, stamp);
-            for (uint64_t s = starting_first[a]; s < starting_first[a + 1]; ++s)
-                add(overlaps[by_target[by_target_first[t] + starting[s]]].q_id, stamp);
-            uint64_t part_bytes = with_fresh(0, false);
-            if (part_bytes > budget) throw WindowOverBudget(t, static_cast<uint32_t>(a), part_bytes, budget);
-            uint64_t part_sum = next_sum;
-            bool part_quality = next_quality;
-            uint64_t b = a + 1;
-            for (; b < n_windows; ++b) {   // grow while the next window's new reads fit
-                fresh.clear();
-                for (uint64_t s = starting_first[b]; s < starting_first[b + 1]; ++s)
-                    add(overlaps[by_target[by_target_first[t] + starting[s]]].q_id, stamp);
-                const uint64_t grown = with_fresh(part_sum, part_quality);
-                if (grown > budget) break;
-                part_bytes = grown;
-                part_sum = next_sum;
-                part_quality = next_quality;
-            }
-            std::vector<uint64_t> local(carry);
-            for (uint64_t s = starting_first[a]; s < starting_first[b]; ++s) local.push_back(starting[s]);
-            std::sort(local.begin(), local.end());   // file order: by_target keeps it
-            g.first_target.push_back(t);
-            g.bytes.push_back(part_bytes);
-            g.first_window.push_back(static_cast<uint32_t>(a));
-            g.end_window.push_back(static_cast<uint32_t>(b));
-            part_overlaps.resize(g.size());
-            carry.clear();
-            for (uint64_t i : local) {
-                part_overlaps.back().push_back(by_target[by_target_first[t] + i]);
-                if (last_w[i] >= b) carry.push_back(i);
-            }
-            a = b;
-        }
-    };
-
-    bool open = false;   // the last group takes further targets
+    ReadGroups plan;
+    std::vector<ReadGroups::Group>& groups = plan.groups;
+    OpenStore store(sequences);
+    std::vector<uint32_t> ids;   // the sequences a target, or a window, would add to the store
+    bool open = false;           // the last group takes further targets
     for (uint64_t t = 0; t < targets_size; ++t) {
-        uint64_t bytes = open ? with_target(t, g.size(), sum, any_quality) : 0;
-        if (!open || bytes > budget) {   // t starts a group of its own
-            for (uint32_t id : fresh) member_of[id] = 0;
-            bytes = with_target(t, g.size() + 1, 0, false);
-            if (bytes > budget) {
-                if (window_length == 0) throw TargetOverBudget(t, bytes, budget);
-                for (uint32_t id : fresh) member_of[id] = 0;   // the first part takes the stamp t tried
-                split_target(t, bytes);
-                open = false;
+        ids.assign(1, static_cast<uint32_t>(t));
+        for (uint64_t k = by_target_first[t]; k < by_target_first[t + 1]; ++k) ids.push_back(overlaps[by_target[k]].q_id);
+        if (open) {
+            const uint64_t bytes = store.bytes_with(ids);
+            if (bytes <= budget) {
+                store.commit();
+                groups.back().end_target = t + 1;
+                groups.back().bytes = bytes;
                 continue;
             }
-            g.first_target.push_back(t);
-            g.bytes.push_back(0);
-            g.first_window.push_back(0);
-            g.end_window.push_back(0);
-            open = true;
         }
-        g.bytes.back() = bytes;
-        sum = next_sum;
-        any_quality = next_quality;
-    }
-    g.first_target.push_back(targets_size);
-    part_overlaps.resize(g.size());
+        store.open();   // t starts a group of its own
+        const uint64_t bytes = store.bytes_with(ids);
+        open = bytes <= budget;
+        if (open) {
+            store.commit();
+            groups.push_back({t, t + 1, 0, ReadGroups::kAllWindows, bytes});
+            continue;
+        }
+        const uint64_t n = window_length > 0 ? n_windows(t) : 0;
+        if (n == 0) throw TargetOverBudget(t, bytes, budget);
 
-    /* each group's overlaps in their original order: a whole group's by a stable counting sort by group, a part's as
-     * planned; an overlap is aligned by its only group, or by the first part it is in */
-    std::vector<uint64_t> group_of(targets_size);
-    for (size_t k = 0; k < g.size(); ++k)
-        std::fill(group_of.begin() + g.first_target[k], group_of.begin() + g.first_target[k + 1], k);
-    g.overlap_first.assign(g.size() + 1, 0);
-    for (const Overlap& o : overlaps)
-        if (!split[o.t_id]) ++g.overlap_first[group_of[o.t_id] + 1];
-    for (size_t k = 0; k < g.size(); ++k) g.overlap_first[k + 1] += g.overlap_first[k] + part_overlaps[k].size();
-    g.overlap_order.resize(g.overlap_first.back());
-    g.aligned_in.assign(overlaps.size(), ~0ull);
-    std::vector<uint64_t> at(g.overlap_first.begin(), g.overlap_first.end() - 1);
-    for (uint64_t k = 0; k < overlaps.size(); ++k) {
-        if (split[overlaps[k].t_id]) continue;
-        g.aligned_in[k] = group_of[overlaps[k].t_id];
-        g.overlap_order[at[g.aligned_in[k]]++] = k;
-    }
-    for (size_t p = 0; p < g.size(); ++p) {
-        for (uint64_t k : part_overlaps[p]) {
-            if (g.aligned_in[k] == ~0ull) g.aligned_in[k] = p;
-            g.overlap_order[at[p]++] = k;
+        /* t alone is over the budget: its windows are cut greedily into maximal parts [a, b), each a group of its own */
+        std::vector<std::array<uint64_t, 3>> spans;   // (first window, last window, overlap) of t's overlaps
+        for (uint64_t k = by_target_first[t]; k < by_target_first[t + 1]; ++k) {
+            const auto w = touched(overlaps[by_target[k]]);
+            spans.push_back({w.first, w.second, by_target[k]});
+        }
+        std::sort(spans.begin(), spans.end());
+        std::vector<size_t> carry;   // the spans of the last part that reach past it
+        size_t s = 0;                // spans[s..]: those that start in a window no part has yet
+        for (uint64_t a = 0, b; a < n; a = b) {
+            store.open();
+            ids.assign(1, static_cast<uint32_t>(t));
+            for (size_t i : carry) ids.push_back(overlaps[spans[i][2]].q_id);
+            const size_t part_first = s;
+            uint64_t part_bytes = 0;
+            for (b = a; b < n; ++b) {   // window b joins while the store fits
+                size_t e = s;
+                for (; e < spans.size() && spans[e][0] == b; ++e) ids.push_back(overlaps[spans[e][2]].q_id);
+                const uint64_t joined = store.bytes_with(ids);
+                if (joined > budget) {
+                    if (b == a) throw WindowOverBudget(t, static_cast<uint32_t>(a), joined, budget);
+                    break;
+                }
+                store.commit();
+                part_bytes = joined;
+                s = e;
+                ids.clear();
+            }
+            groups.push_back({t, t + 1, static_cast<uint32_t>(a), static_cast<uint32_t>(b), part_bytes});
+            carry.erase(std::remove_if(carry.begin(), carry.end(), [&](size_t i) { return spans[i][1] < b; }),
+                        carry.end());
+            for (size_t i = part_first; i < s; ++i)
+                if (spans[i][1] >= b) carry.push_back(i);
         }
     }
-    return g;
+
+    /* The groups that hold overlap o, [first, end): those of its target whose windows it touches.  Groups come in
+     * (target, window) order, so both are contiguous runs. */
+    auto holders = [&](const Overlap& o) {
+        const auto w = touched(o);
+        using Group = ReadGroups::Group;
+        auto first = std::partition_point(groups.begin(), groups.end(),
+                                          [&](const Group& x) { return x.end_target <= o.t_id; });
+        auto end = std::partition_point(first, groups.end(), [&](const Group& x) { return x.first_target <= o.t_id; });
+        first = std::partition_point(first, end, [&](const Group& x) { return x.end_window <= w.first; });
+        end = std::partition_point(first, end, [&](const Group& x) { return x.first_window <= w.second; });
+        return std::make_pair(static_cast<uint64_t>(first - groups.begin()), static_cast<uint64_t>(end - groups.begin()));
+    };
+    /* every group's overlaps in file order (a stable counting sort by group), and the first group of each aligns it */
+    plan.overlap_first.assign(groups.size() + 1, 0);
+    plan.aligned_in.resize(overlaps.size());
+    for (uint64_t k = 0; k < overlaps.size(); ++k) {
+        const auto h = holders(overlaps[k]);
+        plan.aligned_in[k] = h.first;
+        for (uint64_t g = h.first; g < h.second; ++g) ++plan.overlap_first[g + 1];
+    }
+    for (size_t g = 0; g < groups.size(); ++g) plan.overlap_first[g + 1] += plan.overlap_first[g];
+    plan.overlap_order.resize(plan.overlap_first.back());
+    std::vector<uint64_t> at(plan.overlap_first.begin(), plan.overlap_first.end() - 1);
+    for (uint64_t k = 0; k < overlaps.size(); ++k) {
+        const auto h = holders(overlaps[k]);
+        for (uint64_t g = h.first; g < h.second; ++g) plan.overlap_order[at[g]++] = k;
+    }
+    return plan;
 }
 
 void Polisher::polish_groups(std::vector<Overlap>& overlaps, const std::function<void(const PolishedSequence&)>& sink,
@@ -871,85 +868,56 @@ void Polisher::polish_groups(std::vector<Overlap>& overlaps, const std::function
         }
         read_store_bytes = smallest / 2;
     }
-    const ReadGroups groups =
+    const ReadGroups plan =
         plan_read_groups(targets_size_, sequences_, overlaps, read_store_bytes, split_targets ? window_length_ : 0);
 
     resident_reads_ = true;
     group_store_bytes_.clear();
     group_windows_.clear();
     group_aligned_.clear();
-    stitch_data_.clear();
-    stitch_polished_ = 0;
-    /* RC:i: counts every overlap onto a target, whichever parts of it they touch (a whole group recounts the same) */
-    targets_coverages_.assign(targets_size_, 0);
-    for (const Overlap& o : overlaps) ++targets_coverages_[o.t_id];
+    failed_overlaps_.clear();
+    count_coverages(overlaps);
     std::vector<uint64_t> last_group(overlaps.size(), 0);   // the last group an overlap is in
-    for (size_t g = 0; g < groups.size(); ++g)
-        for (uint64_t k = groups.overlap_first[g]; k < groups.overlap_first[g + 1]; ++k)
-            last_group[groups.overlap_order[k]] = g;
-    std::vector<size_t> failed_overlaps, failed_windows;   // whole-run indices
-    uint64_t windows_before = 0;                           // windows of the groups before this one
-    for (size_t g = 0; g < groups.size(); ++g) {
-        const uint64_t first = groups.first_target[g];
-        const uint64_t end = groups.is_part(g) ? first + 1 : groups.first_target[g + 1];
-        /* the group's overlaps, in their original order, moved out and back */
-        std::vector<Overlap> subset;
-        subset.reserve(groups.overlap_first[g + 1] - groups.overlap_first[g]);
-        for (uint64_t k = groups.overlap_first[g]; k < groups.overlap_first[g + 1]; ++k)
-            subset.push_back(std::move(overlaps[groups.overlap_order[k]]));
-        auto global_overlap = [&](size_t local) { return groups.overlap_order[groups.overlap_first[g] + local]; };
+    for (size_t g = 0; g < plan.size(); ++g)
+        for (uint64_t k = plan.overlap_first[g]; k < plan.overlap_first[g + 1]; ++k) last_group[plan.overlap_order[k]] = g;
+    Stitch stitch;
+    std::vector<size_t> failed_windows;   // whole-run indices
+    uint64_t windows_before = 0;          // windows of the groups before this one
+    for (size_t g = 0; g < plan.size(); ++g) {
+        const ReadGroups::Group& group = plan.groups[g];
+        const std::vector<uint64_t> ids(plan.overlap_order.begin() + plan.overlap_first[g],
+                                        plan.overlap_order.begin() + plan.overlap_first[g + 1]);
 
         /* the store first, on every distinct device: the batch objects then size themselves from what is left */
-        store_members_.assign(sequences_.size(), 0);
-        std::fill(store_members_.begin() + first, store_members_.begin() + end, 1);
-        for (const Overlap& o : subset) store_members_[o.q_id] = 1;
+        std::vector<uint8_t> members(sequences_.size(), 0);
+        std::fill(members.begin() + group.first_target, members.begin() + group.end_target, 1);
+        for (uint64_t k : ids) members[overlaps[k].q_id] = 1;
         run_stage([&] {
-            for (uint32_t d : distinct) read_store(d);
+            for (uint32_t d : distinct) read_store(d, members);
         }, [&] { release_read_stores(); });
         group_store_bytes_.push_back(rp_reads_bytes(stores_.front().second));
 
-        /* the overlaps this group aligns: every one of a whole group, those of a part that no earlier part aligned (an
-         * overlap the device refused, or one without a match in any window, has no breaking points either) */
-        std::vector<Overlap> todo;
-        std::vector<uint64_t> todo_ids;
-        for (uint64_t k = 0; k < subset.size(); ++k) {
-            if (groups.aligned_in[global_overlap(k)] != g) continue;
-            todo.push_back(std::move(subset[k]));
-            todo_ids.push_back(global_overlap(k));
-        }
-        failed_overlaps_.clear();
-        overlap_ids_ = todo_ids.data();   // warnings name whole-run indices
-        group_aligned_.push_back(find_overlap_breaking_points(todo));
-        overlap_ids_ = nullptr;
-        for (size_t k : failed_overlaps_) failed_overlaps.push_back(todo_ids[k]);
-        for (uint64_t k = 0, j = 0; k < subset.size(); ++k)
-            if (groups.aligned_in[global_overlap(k)] == g) subset[k] = std::move(todo[j++]);
+        /* the overlaps no earlier group holds (one the device refused, or one without a match in any window, has no
+         * breaking points either, so they cannot tell) */
+        std::vector<uint64_t> todo;
+        for (uint64_t k : ids)
+            if (plan.aligned_in[k] == g) todo.push_back(k);
+        group_aligned_.push_back(find_overlap_breaking_points(overlaps, todo));
 
         windows_.clear();
-        if (groups.is_part(g)) {
-            build_windows(subset, first, groups.first_window[g], groups.end_window[g]);
-        } else {
-            build_windows(subset, first, end);
-        }
+        build_windows(overlaps, ids, group.first_target, group.end_target, group.first_window, group.end_window);
         failed_windows_.clear();
-        consensus(sink, drop_unpolished_sequences, memory, banded, true, true);
+        consensus(sink, stitch, drop_unpolished_sequences, memory, banded, true, true);
         for (size_t w : failed_windows_) failed_windows.push_back(windows_before + w);
         group_windows_.emplace_back(windows_before, windows_before + windows_.size());
         windows_before += windows_.size();
 
         release_read_stores();
-        for (uint64_t k = 0; k < subset.size(); ++k) {
-            /* a split target's overlap is done with its breaking points after its last part */
-            if (groups.is_part(g) && last_group[global_overlap(k)] == g)
-                std::vector<std::pair<uint32_t, uint32_t>>().swap(subset[k].breaking_points_);
-            overlaps[global_overlap(k)] = std::move(subset[k]);
-        }
+        for (uint64_t k : ids)
+            if (last_group[k] == g) std::vector<std::pair<uint32_t, uint32_t>>().swap(overlaps[k].breaking_points_);
     }
-    store_members_.clear();
     windows_.clear();
-    std::sort(failed_overlaps.begin(), failed_overlaps.end());
-    failed_overlaps_ = std::move(failed_overlaps);
-    failed_windows_ = std::move(failed_windows);   // groups in target order: already sorted
+    failed_windows_ = std::move(failed_windows);   // groups in target and window order: already sorted
 }
 
 }  // namespace racon_b200
@@ -1255,15 +1223,21 @@ extern "C" void rp_mirror_last_grouped_run_windows(uint64_t* group_windows, uint
 }
 
 /* Host-only hook of plan_read_groups: n_seq sequences (the first n_targets are the targets) of length[i], with a quality
- * string when has_quality[i]; overlap k runs from sequence q_id[k] onto target t_id[k].  Outputs (capacities: n_targets + 1
- * groups at most): group g = targets [first_target[g], first_target[g + 1]), predicted store bytes[g], and its overlaps
- * overlap_order[overlap_first[g] .. overlap_first[g + 1]) (n_overlaps entries in all).  Returns the number of groups, or
- * -1 with the error in err (a target over the budget). */
+ * string when has_quality[i]; overlap k runs from sequence q_id[k] onto target t_id[k], over its target span
+ * [t_begin[k], t_end[k]).  window_length = 0 does not split targets, and t_begin / t_end may then be NULL.
+ * sizes[0] = groups, sizes[1] = entries of overlap_order (an overlap is in every part it touches); with every output
+ * NULL only sizes is written.  Outputs: group g = targets [first_target[g], first_target[g + 1]) (first_target has
+ * sizes[0] + 1 entries; a part's next entry is its own target until its target's last part), predicted store bytes[g],
+ * its overlaps overlap_order[overlap_first[g] .. overlap_first[g + 1]), its windows [first_window[g], end_window[g])
+ * when it is a part (0, 0 for whole targets), and per overlap the group that aligns it.  Returns the number of groups,
+ * or -1 with the error in err (a target, or with a window length a window, over the budget). */
 extern "C" int64_t rp_mirror_plan_read_groups(uint64_t n_targets, uint32_t n_seq, const uint32_t* length,
                                               const uint8_t* has_quality, uint64_t n_overlaps, const uint32_t* q_id,
-                                              const uint32_t* t_id, uint64_t budget, uint64_t* first_target,
-                                              uint64_t* bytes, uint64_t* overlap_first, uint64_t* overlap_order,
-                                              char* err, uint32_t err_cap) {
+                                              const uint32_t* t_id, const uint32_t* t_begin, const uint32_t* t_end,
+                                              uint32_t window_length, uint64_t budget, uint64_t* sizes,
+                                              uint64_t* first_target, uint64_t* bytes, uint64_t* overlap_first,
+                                              uint64_t* overlap_order, uint32_t* first_window, uint32_t* end_window,
+                                              uint64_t* aligned_in, char* err, uint32_t err_cap) {
     using namespace racon_b200;
     static const char kQuality[] = "";   // stands for "has a quality string": the planner only tests for null
     std::vector<SequenceView> seqs(n_seq);
@@ -1272,63 +1246,27 @@ extern "C" int64_t rp_mirror_plan_read_groups(uint64_t n_targets, uint32_t n_seq
     for (uint64_t k = 0; k < n_overlaps; ++k) {
         ovl[k].q_id = q_id[k];
         ovl[k].t_id = t_id[k];
+        ovl[k].t_begin = window_length ? t_begin[k] : 0;
+        ovl[k].t_end = window_length ? t_end[k] : 0;
     }
     try {
-        const ReadGroups g = plan_read_groups(n_targets, seqs, ovl, budget);
-        std::copy(g.first_target.begin(), g.first_target.end(), first_target);
-        std::copy(g.bytes.begin(), g.bytes.end(), bytes);
-        std::copy(g.overlap_first.begin(), g.overlap_first.end(), overlap_first);
-        std::copy(g.overlap_order.begin(), g.overlap_order.end(), overlap_order);
-        return static_cast<int64_t>(g.size());
-    } catch (const std::exception& e) {
-        if (err && err_cap) {
-            std::strncpy(err, e.what(), err_cap - 1);
-            err[err_cap - 1] = '\0';
-        }
-        return -1;
-    }
-}
-
-/* Host-only hook of plan_read_groups with split targets: rp_mirror_plan_read_groups' inputs plus each overlap's target
- * span [t_begin[k], t_end[k]) and the window length.  sizes[0] = groups, sizes[1] = entries of overlap_order (an
- * overlap is in every part it touches); with every output NULL only sizes is written.  Outputs as
- * rp_mirror_plan_read_groups', and per group the windows [first_window[g], end_window[g]) of a part (0, 0 for whole targets), per overlap the group that
- * aligns it.  Returns the number of groups, or -1 with the error in err (a target with no window, or a window, over the
- * budget). */
-extern "C" int64_t rp_mirror_plan_split_read_groups(uint64_t n_targets, uint32_t n_seq, const uint32_t* length,
-                                                    const uint8_t* has_quality, uint64_t n_overlaps,
-                                                    const uint32_t* q_id, const uint32_t* t_id,
-                                                    const uint32_t* t_begin, const uint32_t* t_end,
-                                                    uint32_t window_length, uint64_t budget, uint64_t* sizes,
-                                                    uint64_t* first_target, uint64_t* bytes, uint64_t* overlap_first,
-                                                    uint64_t* overlap_order, uint32_t* first_window,
-                                                    uint32_t* end_window, uint64_t* aligned_in, char* err,
-                                                    uint32_t err_cap) {
-    using namespace racon_b200;
-    static const char kQuality[] = "";
-    std::vector<SequenceView> seqs(n_seq);
-    for (uint32_t i = 0; i < n_seq; ++i) seqs[i] = SequenceView{nullptr, has_quality[i] ? kQuality : nullptr, length[i]};
-    std::vector<Overlap> ovl(n_overlaps);
-    for (uint64_t k = 0; k < n_overlaps; ++k) {
-        ovl[k].q_id = q_id[k];
-        ovl[k].t_id = t_id[k];
-        ovl[k].t_begin = t_begin[k];
-        ovl[k].t_end = t_end[k];
-    }
-    try {
-        const ReadGroups g = plan_read_groups(n_targets, seqs, ovl, budget, window_length);
-        sizes[0] = g.size();
-        sizes[1] = g.overlap_order.size();
+        const ReadGroups plan = plan_read_groups(n_targets, seqs, ovl, budget, window_length);
+        sizes[0] = plan.size();
+        sizes[1] = plan.overlap_order.size();
         if (first_target) {
-            std::copy(g.first_target.begin(), g.first_target.end(), first_target);
-            std::copy(g.bytes.begin(), g.bytes.end(), bytes);
-            std::copy(g.overlap_first.begin(), g.overlap_first.end(), overlap_first);
-            std::copy(g.overlap_order.begin(), g.overlap_order.end(), overlap_order);
-            std::copy(g.first_window.begin(), g.first_window.end(), first_window);
-            std::copy(g.end_window.begin(), g.end_window.end(), end_window);
-            std::copy(g.aligned_in.begin(), g.aligned_in.end(), aligned_in);
+            for (size_t g = 0; g < plan.size(); ++g) {
+                const ReadGroups::Group& group = plan.groups[g];
+                first_target[g] = group.first_target;
+                bytes[g] = group.bytes;
+                first_window[g] = group.first_window;
+                end_window[g] = group.end_window == ReadGroups::kAllWindows ? 0 : group.end_window;
+            }
+            first_target[plan.size()] = n_targets;
+            std::copy(plan.overlap_first.begin(), plan.overlap_first.end(), overlap_first);
+            std::copy(plan.overlap_order.begin(), plan.overlap_order.end(), overlap_order);
+            std::copy(plan.aligned_in.begin(), plan.aligned_in.end(), aligned_in);
         }
-        return static_cast<int64_t>(g.size());
+        return static_cast<int64_t>(plan.size());
     } catch (const std::exception& e) {
         if (err && err_cap) {
             std::strncpy(err, e.what(), err_cap - 1);

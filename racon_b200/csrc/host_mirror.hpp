@@ -219,27 +219,28 @@ private:
 };
 
 /* ---- target groups: polishing a read set larger than one device's memory -------------------------------------------
- * A group is a contiguous range of targets together with the read store of exactly the sequences it needs: its targets
- * and every read with an overlap onto one of them.  Its store costs read_store_bytes() of those sequences
- * (rp_reads_bytes' rule).  A read needed by two groups (racon -f, reads spanning contig ends) is counted in both. */
+ * A group is windows [first_window, end_window) of each target in [first_target, end_target), together with the read
+ * store of exactly the sequences it needs: its targets and every read whose overlap onto one of them touches one of
+ * those windows.  A group of whole targets has every window of its targets (end_window = kAllWindows); a part of a split
+ * target is one target's windows [a, b).  Its store costs read_store_bytes() of those sequences (rp_reads_bytes' rule).
+ * A read needed by two groups (racon -f, reads spanning contig ends, overlaps across a part boundary) is counted in both. */
 uint64_t read_store_bytes(uint64_t sum_of_lengths, bool any_quality);
 
 struct ReadGroups {
-    /* group g = targets [first_target[g], first_target[g + 1]); a part (below) is of target first_target[g] */
-    std::vector<uint64_t> first_target;
-    std::vector<uint64_t> bytes;           // predicted rp_reads_bytes of group g's store
+    static constexpr uint32_t kAllWindows = ~0u;
+    struct Group {
+        uint64_t first_target, end_target;
+        uint32_t first_window, end_window;
+        uint64_t bytes;   // predicted rp_reads_bytes of the group's store
+    };
+    std::vector<Group> groups;
     /* group g's overlaps, as indices into the overlaps, in their original (file) order: a window's layer order is the
-     * order of its overlaps, and it decides the consensus */
-    std::vector<uint64_t> overlap_first;   // group g = overlap_order[overlap_first[g] .. overlap_first[g + 1])
-    std::vector<uint64_t> overlap_order;
-    /* A part (split targets only): group g is windows [first_window[g], end_window[g]) of its one target, and its
-     * overlaps are those whose target span touches one of them — an overlap across two parts is in both.  A group of
-     * whole targets has first_window[g] = end_window[g] = 0. */
-    std::vector<uint32_t> first_window, end_window;
-    /* the group that aligns overlap k: the only group it is in, or the first part it touches */
+     * order of its overlaps, and it decides the consensus.  They are the overlaps onto its targets whose target span
+     * touches one of its windows.  group g = overlap_order[overlap_first[g] .. overlap_first[g + 1]) */
+    std::vector<uint64_t> overlap_first, overlap_order;
+    /* the group that aligns overlap k: the first group that holds it */
     std::vector<uint64_t> aligned_in;
-    size_t size() const { return bytes.size(); }
-    bool is_part(size_t g) const { return end_window[g] > 0; }
+    size_t size() const { return groups.size(); }
 };
 
 /* A single target whose own store exceeds the budget: it cannot be polished under that budget in one group. */
@@ -265,8 +266,9 @@ struct WindowOverBudget : TargetOverBudget {
  * Throws TargetOverBudget.
  * window_length > 0 splits targets: a target whose own store exceeds the budget closes the open group and is cut into
  * maximal parts of consecutive windows (window_length bases each, as the polisher builds them), each a group of its
- * own; an overlap touches windows t_begin / window_length .. (t_end - 1) / window_length.  Targets that fit get the
- * groups they get without splitting.  Throws WindowOverBudget when one window does not fit. */
+ * own; an overlap touches windows t_begin / window_length .. (t_end - 1) / window_length of its target (clamped to its
+ * last window; an empty span touches its first window).  Targets that fit get the groups they get without splitting.
+ * Throws WindowOverBudget when one window does not fit. */
 ReadGroups plan_read_groups(uint64_t targets_size, const std::vector<SequenceView>& sequences,
                             const std::vector<Overlap>& overlaps, uint64_t budget, uint32_t window_length = 0);
 
@@ -295,12 +297,6 @@ public:
     void initialize(std::vector<Overlap>& overlaps);
     /* the window-building half of initialize() alone, for overlaps whose breaking points are already known */
     void build_windows(const std::vector<Overlap>& overlaps);
-    /* the same for targets [first_target, end_target) alone, whose overlaps those are */
-    void build_windows(const std::vector<Overlap>& overlaps, uint64_t first_target, uint64_t end_target);
-    /* the same for windows [first_window, end_window) of one target alone, from the overlaps that touch them: layers
-     * that fall in the target's other windows are left out, and the target's RC:i: count is not touched */
-    void build_windows(const std::vector<Overlap>& overlaps, uint64_t target, uint32_t first_window,
-                       uint32_t end_window);
     void polish(std::vector<PolishedSequence>& dst, bool drop_unpolished_sequences);
     /* Streaming form (polisher.cpp:504-537 + main.cpp:159-161 as a consumer overlapped with the compute): two batch
      * objects per lane stay in flight; while they run on the GPUs the finished windows are stitched in window order, and
@@ -311,16 +307,16 @@ public:
     void polish_streaming(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
                           size_t memory = 0, bool banded = false, bool resident_reads = false);
     /* initialize + polish_streaming(resident_reads = true) in target groups (plan_read_groups): for each group in target
-     * order, its store goes to every distinct device, its overlaps are aligned, its windows built and polished, its records
-     * streamed to `sink`, and its store released.  `read_store_bytes` = budget per device (0 = half of the smallest free
-     * memory of the devices, read before anything is allocated).  The overlaps come from load_input (filter and window
-     * type over the whole input); failed_overlaps / failed_windows keep their whole-run indices.  With one group the
-     * output is that of initialize + polish_streaming.  Throws TargetOverBudget before any device work.
-     * split_targets: a target whose own store exceeds the budget is polished in parts (plan_read_groups with the window
-     * length): each overlap is aligned once, in the first part it touches, and keeps its breaking points until its last
-     * part has built its windows; a part builds only its windows, and the target's record is stitched across its parts
-     * and goes to `sink` after its last window, with RC:i: counting every overlap onto the target.  The output is still
-     * that of one pass.  Throws WindowOverBudget (before any device work) when one window does not fit. */
+     * order, its store goes to every distinct device, the overlaps it aligns (aligned_in) are aligned, its windows built
+     * from its overlaps and polished, its records streamed to `sink`, and its store released; an overlap's breaking points
+     * are freed after its last group.  `read_store_bytes` = budget per device (0 = half of the smallest free memory of
+     * the devices, read before anything is allocated).  The overlaps come from load_input (filter and window type over
+     * the whole input); failed_overlaps / failed_windows keep their whole-run indices, RC:i: counts every overlap onto
+     * the target, and the stitch carries from one group to the next, so a target's record goes to `sink` after its last
+     * window.  With one group the output is that of initialize + polish_streaming.  Throws TargetOverBudget before any
+     * device work.  split_targets: a target whose own store exceeds the budget is polished in parts (plan_read_groups
+     * with the window length), with the output of one pass; throws WindowOverBudget (before any device work) when one
+     * window does not fit. */
     void polish_groups(std::vector<Overlap>& overlaps, const std::function<void(const PolishedSequence&)>& sink,
                        bool drop_unpolished_sequences, size_t memory, bool banded, uint64_t read_store_bytes,
                        bool split_targets = false);
@@ -343,14 +339,28 @@ private:
     const Polisher& operator=(const Polisher&) = delete;
     const char* reverse_complement(uint32_t id);
     const char* reverse_quality(uint32_t id);
+    /* the breaking points of overlaps[ids[..]]: those with an alignment (SAM) from it, the others on the device;
+     * returns the number of overlaps sent to the device aligner */
+    size_t find_overlap_breaking_points(std::vector<Overlap>& overlaps, const std::vector<uint64_t>& ids);
     /* the aligner lanes of find_overlap_breaking_points over overlaps[todo[..]] */
-    void align(std::vector<Overlap>& overlaps, const std::vector<size_t>& todo, uint32_t longest);
+    void align(std::vector<Overlap>& overlaps, const std::vector<uint64_t>& todo, uint32_t longest);
+    /* RC:i: of every target: the number of overlaps onto it */
+    void count_coverages(const std::vector<Overlap>& overlaps);
+    /* windows [first_window, end_window) of every target in [first_target, end_target) (polisher.cpp:383-401), appended
+     * to windows_, with the layers of overlaps[ids[..]] that fall in them */
+    void build_windows(const std::vector<Overlap>& overlaps, const std::vector<uint64_t>& ids, uint64_t first_target,
+                       uint64_t end_target, uint32_t first_window, uint32_t end_window);
+    /* the stitch of the target whose windows are being emitted: within a run it carries from one group to the next */
+    struct Stitch {
+        std::string data;
+        uint32_t polished_windows = 0;
+    };
     /* the one batch loop + stitch of polish() and polish_streaming(); `release`: drop every window once stitched.  A
      * hard error in either stage destroys its batch objects and the read stores before the process exits. */
-    void consensus(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
-                   size_t memory, bool banded, bool resident_reads, bool release);
-    void consensus_lanes(const std::function<void(const PolishedSequence&)>& sink, bool drop_unpolished_sequences,
-                         size_t memory, bool banded, bool resident_reads, bool release);
+    void consensus(const std::function<void(const PolishedSequence&)>& sink, Stitch& stitch,
+                   bool drop_unpolished_sequences, size_t memory, bool banded, bool resident_reads, bool release);
+    void consensus_lanes(const std::function<void(const PolishedSequence&)>& sink, Stitch& stitch,
+                         bool drop_unpolished_sequences, size_t memory, bool banded, bool resident_reads, bool release);
     void release_read_stores();
     /* the layers of overlap o in windows [first_window, end_window) of its target, whose window first_window is
      * windows_[first_window_id] (polisher.cpp:405-458) */
@@ -372,14 +382,10 @@ private:
     std::vector<size_t> failed_overlaps_, failed_windows_;
     bool resident_reads_ = false;
     std::vector<std::pair<uint32_t, rp_reads*>> stores_;   // (device, store): one per distinct device, made at first use
-    std::vector<uint8_t> store_members_;   // empty: stores hold every sequence; else those i with store_members_[i]
     std::vector<uint64_t> group_store_bytes_, group_aligned_;
     std::vector<std::pair<uint64_t, uint64_t>> group_windows_;
-    /* the stitch of the target whose windows are being emitted: it carries from one part of a split target to the next */
-    std::string stitch_data_;
-    uint32_t stitch_polished_ = 0;
-    const uint64_t* overlap_ids_ = nullptr;   // while a group is aligned: whole-run index of each overlap of the group
-    const rp_reads* read_store(uint32_t device);
+    /* the store on `device`; made at first use, of the sequences i with members[i] (every sequence when empty) */
+    const rp_reads* read_store(uint32_t device, const std::vector<uint8_t>& members = {});
 };
 
 }  // namespace racon_b200
